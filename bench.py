@@ -32,7 +32,7 @@ def _peaks():
             p = json.load(f)
         return float(p["bf16_tflops_sustained"]), "measured (MEASURED_PEAKS.json bf16_tflops_sustained)"
     except Exception:
-        return 1400.0, "fallback (B200_PROFILING.md sustained bf16)"
+        return 989.0, "H100 SXM data sheet, dense bf16 (700 W card; not a measured peak)"
 
 
 def _masks(B, seed, up=1):
@@ -73,7 +73,7 @@ FLOPS_SEGGPT_FWD = 1589.74e9        # SURVEY.md section 8(d): SegGPT 1-prompt in
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
 
     def __init__(self, index):
         self.rows = []
@@ -121,7 +121,7 @@ class ClockSampler:
 
 def cpu_reference_step_time(threads, reps=1, budget_s=None, min_reps=1):
     """The reference's own CPU path: the UNMODIFIED `models_painter.painter_vit_large_patch16_input896x448_win_dec64_
-    8glb_sl1()` module (staged copy under baseline/_ref, scripts/stage_reference.py; loaded through oracle/ref_loader)
+    8glb_sl1()` module (staged copy under oracle/_ref, scripts/stage_reference.py; loaded through oracle/ref_loader)
     in torch-CPU eager fp32, train mode, B=1 896x448 forward + backward on `threads` host threads.  Falls back to the
     oracle port (kind "port") only if the staged tree is missing.  With `budget_s` the loop stops early once that much
     wall time is spent (after at least `min_reps` steps), so the CPU legs stay bounded whatever --steps is.
@@ -389,13 +389,13 @@ def run_seggpt(args):
                        "parallelism": "single" if world == 1 else f"{world} replicas", "tokens_per_image": 1568,
                        "forward": "one CUDA-graph replay of the whole forward", "kernels_per_forward": int(launches),
                        "eager_ms_per_step": ms_eager,
-                       "l2": "weights (0.74 GB bf16) exceed the 126 MB L2; no explicit flush"},
+                       "l2": "weights (0.74 GB bf16) exceed the 50 MB L2; no explicit flush"},
             "e2e": {"value": world * 1e3 / ms_e2e, "unit": "images/s", "ms_per_step": ms_e2e,
                     "h2d_bytes_per_step": int(img.nbytes + tgt.nbytes), "d2h_bytes_per_step": int(out.numel() * 8),
                     "call": "painter_b200.seggpt_engine.run_one_image(img, tgt, model, device): numpy float64 canvases in, "
                             "de-normalised [448,448,3] float64 result on the host out (wall clock incl. both copies)"},
             "gpu_launches": int(launches) * steps * 5,
-            "roofline": {"bound": "tensor", "kernel": "whole forward (tcgen05 GEMMs + fused attention), one graph replay",
+            "roofline": {"bound": "tensor", "kernel": "whole forward (wgmma GEMMs + fused attention), one graph replay",
                          "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
                          "peak_source": peak_src, "algorithmic_per_launch": FLOPS_SEGGPT_FWD, "traffic": None},
             "clocks": clk,
@@ -414,6 +414,27 @@ def run_seggpt(args):
         print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()
+
+
+DUMP_MAX_BYTES = 48 << 20
+
+
+def dump_outputs(d, outs):
+    """Write each output as d/<name>.npy: the loss in float64, the rest in float32.  An array larger than
+    DUMP_MAX_BYTES is replaced by a fixed, seeded sample of its flattened elements (the same sorted indices every run:
+    torch.randperm with seed 0)."""
+    import numpy as np
+    import torch
+    os.makedirs(d, exist_ok=True)
+    for name, t in outs.items():
+        a = t.detach().double() if name == "loss" else t.detach().float()
+        a = a.cpu().numpy()
+        if a.nbytes > DUMP_MAX_BYTES:
+            n = DUMP_MAX_BYTES // a.itemsize
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randperm(a.size, generator=g)[:n].sort().values.numpy()
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(d, f"{name}.npy"), a)
 
 
 def main():
@@ -447,6 +468,9 @@ def main():
                     help="1: the e2e step is painter_b200.train_utils.GraphedTrainStep (forward + backward + AdamW as one "
                          "CUDA-graph replay; N = 1 with the pk optimizer); 0: the reference loop's eager launches")
     ap.add_argument("--no-optimizer", action="store_true", help="diagnostic only; the reported step includes AdamW")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step returned (loss, pred, mask) as "
+                         "DIR/<name>.npy (float32 / float64; pred as a fixed, seeded sample when it exceeds 48 MB)")
     args = ap.parse_args()
     if args.workload == "seggpt":
         return run_seggpt(args)
@@ -511,7 +535,7 @@ def main():
     resident = [t.to(dev) for t in host]
     h2d_bytes = sum(t.numel() * t.element_size() for t in host)
 
-    # per-launch timing of the dominant kernel (the tcgen05 GEMM) with CUDA events on the launching stream
+    # per-launch timing of the dominant kernel (the wgmma GEMM) with CUDA events on the launching stream
     gemm_log = []
     orig_gemm = ops.gemm
     record = {"on": False}
@@ -534,10 +558,14 @@ def main():
     import painter_b200.engine as eng
     eng.ops.gemm = timed_gemm
 
-    def step(batch, read_loss):
+    last_out = {}
+
+    def step(batch, read_loss, keep=False):
         imgs, tgts, mask, valid = batch
         with torch.autocast("cuda", dtype=torch.bfloat16):
-            loss, _, _ = net(imgs, tgts, bool_masked_pos=mask, valid=valid)
+            loss, pred, out_mask = net(imgs, tgts, bool_masked_pos=mask, valid=valid)
+        if keep:
+            last_out.update(loss=loss.detach(), pred=pred.detach(), mask=out_mask.detach())
         loss.backward()
         if not args.no_optimizer:
             opt.step()
@@ -552,8 +580,7 @@ def main():
     # End to end the step runs the way a user of painter_b200 runs it: train_utils.GraphedTrainStep = the same
     # forward + backward + AdamW captured once and replayed as ONE CUDA graph per iteration (single GPU, FusedAdamW).
     # The device-resident region below stays eager - its GEMM launches carry CUDA events - and so does the reference
-    # loop reported next to the e2e figure.  (Measured: the replay is worth 0.5-0.8 % here; the eager step is already
-    # GPU-bound, its ~2.7 us kernel boundaries are not launch latency - profiles/r02_step_timeline_warm.txt.)
+    # loop reported next to the e2e figure.
     gstep = None
     if args.graph and world == 1 and args.optimizer == "pk" and not args.no_optimizer:
         from painter_b200.train_utils import GraphedTrainStep
@@ -567,8 +594,7 @@ def main():
         clocks.start()
     # ---------------- timed region 1: device-resident inputs ----------------
     # The per-launch CUDA events around the GEMMs live inside the timed region, but on two of its steps only (the
-    # first and the middle one): ~340 event pairs per step cost ~1.6 ms of stream bubbles (scripts/step_timeline.py:
-    # 62.6 ms per step without them against 64.2 ms with events on every step).
+    # first and the middle one): events around every launch would add stream bubbles to every step.
     sampled = {0, args.steps // 2}
     n0 = _lib.launch_count()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -576,9 +602,11 @@ def main():
     e0.record()
     for i in range(args.steps):
         record["on"] = i in sampled
-        step(resident, False)
+        step(resident, False, keep=bool(args.dump_outputs) and i == args.steps - 1)
     e1.record()
     sync()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_out)
     launches = _lib.launch_count() - n0
     record["on"] = False
     ms_total = e0.elapsed_time(e1)
@@ -673,14 +701,6 @@ def main():
                       f"TF/s={f / t / 1e9:.0f}", file=sys.stderr)
         peak, peak_src = _peaks()
         achieved = flops / (gms / 1e3) / 1e12 if gms > 0 else 0.0
-        traffic = None      # DRAM bytes per launch of the GEMM kernel, from the committed ncu --set full capture
-        for name in ("r02_ncu_gemm_traffic.json", "r01_ncu_gemm_traffic.json"):
-            try:
-                with open(os.path.join(ROOT, "profiles", name)) as f:
-                    traffic = json.load(f)["avg_dram_bytes_per_launch"]
-                break
-            except (OSError, KeyError, ValueError):
-                continue
         line = {
             "metric": wl["metric"], "value": value, "unit": "images/s",
             "n_gpus": world, "steps": args.steps, "warmup": W_steps, "ms_per_step": ms_step,
@@ -697,7 +717,7 @@ def main():
                        "data_parallel": "single" if world == 1 else (
                            "painter_b200.dist_utils.GradSync (arena buckets, NCCL all-reduce from backward)"
                            if args.dp == "own" else "torch DistributedDataParallel"),
-                       "l2": "per-step working set (1.5 GB weights + >10 GB activations) far exceeds the 126 MB L2; "
+                       "l2": "per-step working set (1.5 GB weights + >10 GB activations) far exceeds the 50 MB L2; "
                              "no explicit flush"},
             "e2e": {"value": e2e_val, "unit": "images/s", "h2d_bytes_per_step": h2d_bytes, "d2h_bytes_per_step": 4,
                     "ms_per_step": ms_e2e / args.steps,
@@ -713,15 +733,22 @@ def main():
                     "pipelined_note": "same work with data_utils.DevicePrefetcher (copies one step ahead on a side "
                                       "stream) and each step's loss read back one step later (no per-step drain)"},
             "gpu_launches": int(launches),
-            "roofline": {"bound": "tensor", "kernel": "pk::gemm_bf16_kernel (tcgen05 GEMM, all linear layers fwd/bwd)",
+            "roofline": {"bound": "tensor", "kernel": "pk::gemm_bf16_kernel (wgmma GEMM, all linear layers fwd/bwd)",
                          "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
                          "frac": achieved / peak if peak else None, "peak_source": peak_src,
-                         "launches": len(gemm_log), "share_of_step": gms / (ms_step * len(sampled)), "traffic": traffic,
+                         "launches": len(gemm_log), "share_of_step": gms / (ms_step * len(sampled)),
                          "algorithmic_per_launch": flops / max(len(gemm_log), 1),
                          "step_mfu": value / world * wl["flops"] / 1e12 / peak},
             "clocks": clk, "loss": last_loss,
         }
         if world == 1 and not args.no_cpu_baseline and args.workload == "train":
+            # the comparator needs most of an 80 GB device: release the timed path's model, optimizer state, graph
+            # buffers and batch first
+            import gc
+            gstep = opt = model = net = resident = None
+            last_out.clear()
+            gc.collect()
+            torch.cuda.empty_cache()
             try:
                 line["reference_cuda_eager"] = reference_cuda_eager(dev, host, args.steps)
             except Exception as ex:      # a labelled extra: never let it take the bench line down

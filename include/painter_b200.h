@@ -1,9 +1,9 @@
-/* painter_b200 — C ABI of the B200-native Painter/SegGPT hot path.
+/* painter_b200 — C ABI of the H100-native Painter/SegGPT hot path.
  *
  * The reference (baaivision/Painter) has no FFI layer: its hot path is the Python module
  * Painter/models_painter.py (+ SegGPT/SegGPT_inference/models_seggpt.py, util/vitdet_utils.py), every
  * arithmetic step being a torch op.  Each entry point below replaces one group of those torch call
- * sites (cited per function) with a hand-written sm_100a kernel.  The host-side mirror of the
+ * sites (cited per function) with a hand-written sm_90a kernel.  The host-side mirror of the
  * reference nn.Module API (painter_b200/models_painter.py, models_seggpt.py) calls these through
  * ctypes; see INTEGRATION.md for the binding.
  *
@@ -29,7 +29,7 @@ const char* pk_last_error(void);
 long long pk_launch_count(void);
 
 /* ------------------------------------------------------------------------------------------------
- * Dense contraction on tcgen05 tensor cores:  C[M,N] = A[M,K] . B[N,K]^T   (bf16 x bf16 -> fp32)
+ * Dense contraction on the tensor cores (wgmma):  C[M,N] = A[M,K] . B[N,K]^T   (bf16 x bf16 -> fp32)
  * Replaces every nn.Linear / F.linear on the path (models_painter.py:60-61,76,87 qkv/proj; timm Mlp
  * fc1/fc2 used at :201; decoder_embed :327,423) and their autograd backward (dgrad / wgrad GEMMs).
  *   transA = 0: A stored [M,K] row-major (lda = row stride, elements)   transA = 1: stored [K,M]
@@ -67,14 +67,13 @@ int pk_gemm_bf16(const void* A, const void* B, int M, int N, int K, int lda, int
 /* test hooks: force the GEMM N-tile (64/128/256) or split-K factor; 0 restores the heuristics */
 void pk_gemm_force_bn(int bn);
 void pk_gemm_force_splits(int s);
-/* Host-only views of the GEMM scheduler (schedule tests; no device work).  pk_gemm_plan: out9 = {cta_pair_kernel,
- * BN, row blocks, column blocks, splits, k-blocks per split, stream-K units per cluster, raster group, workers}.
+/* Host-only views of the GEMM scheduler (schedule tests; no device work).  pk_gemm_plan: out9 = {cta_pair_kernel
+ * (always 0: one CTA per 128 x BN tile), BN, row blocks, column blocks, splits, k-blocks per split, stream-K units per
+ * CTA, raster group, workers}.
  * pk_gemm_plan_walk: the (row block, column block, kb0, kb1) items worker `worker` processes, 4 ints each; returns
  * minus the item count. */
 int pk_gemm_plan(int M, int N, int K, int kind, int accumulate, int* out9);
 int pk_gemm_plan_walk(int M, int N, int K, int kind, int accumulate, int worker, int* out4, int max_items);
-/* 0 = single-CTA tiles (128 x BN), 1 = CTA pairs / cta_group::2 (256 x BN) whenever the shape allows */
-void pk_gemm_use_2cta(int on);
 
 /* ------------------------------------------------------------------------------------------------
  * LayerNorm over channels (nn.LayerNorm(eps=1e-6): models_painter.py:193,200 norm1/norm2, :315,:417 final norm).
@@ -222,7 +221,7 @@ int pk_adamw_step_graph(const PkOptTensor* tensors_dev, const int* chunks_dev, i
                         int zero_grad, const float* found_inf, void* stream);
 int pk_grad_sumsq(const PkOptTensor* tensors_dev, const int* chunks_dev, int nchunks, float* out_zeroed, void* stream);
 int pk_droppath_scales(const void* r, int dtype_code, const float* keep, float* out, int n, void* stream);
-/* Persistent kernels (the tcgen05 GEMMs) use at most `n` SMs (0 = all): leaves room for a concurrent NCCL kernel
+/* Persistent kernels (the GEMM) use at most `n` SMs (0 = all): leaves room for a concurrent NCCL kernel
  * so that statically partitioned tiles never run as a second wave (multi-GPU backward).  Returns the old value. */
 int pk_set_sm_budget(int n);
 /* Programmatic dependent launch of the library's hot kernels (default on; PK_PDL=0 in the environment or
@@ -254,7 +253,7 @@ int pk_bilinear_u8(const double* seg, int SH, int SW, uint8_t* dst, int OH, int 
  * fp32-accurate forward mode (north star: within 1e-5 of the reference's fp32 forward, the way
  * seggpt_engine.run_one_image calls the model, seggpt_engine.py:47).  Every fp32 GEMM operand is split into three
  * bf16 terms (h, m, l) and the six significant cross products are evaluated by ONE pk_gemm_bf16 call over operands
- * concatenated along K: A' = [l|m|h|m|h|h], B' = [h|m|l|h|m|h] (K' = 6K, fp32 accumulation in TMEM).
+ * concatenated along K: A' = [l|m|h|m|h|h], B' = [h|m|l|h|m|h] (K' = 6K, fp32 accumulation).
  *  pk_split3                 out bf16 [M, 6K] from x fp32 [M, K] (side_b: 0 = A-side, 1 = B-side order); gelu != 0
  *                            applies the exact erf GELU (timm Mlp act, models_painter.py:201) first
  *  pk_split3_heads           q / k / v of qkv fp32 [B*N, 3C] -> per-(b, head) operands of the attention GEMMs

@@ -1,10 +1,10 @@
 """TEST INFRASTRUCTURE: import the UNMODIFIED reference modules through the shim packages in oracle/shims
 (timm 0.3.2 symbols, import-only detectron2/fairscale/fvcore, torch._six).
 
-The reference tree is looked up at $PAINTER_REFERENCE, then /root/reference (the authoring container), then the
-staged byte-for-byte copy under baseline/_ref/ (scripts/stage_reference.py; git-ignored, travels to the GPU box with
-the gpurun snapshot).  Nothing in the product path (painter_b200/*) imports this file: only tests/, the
-`--impl reference` / cpu_baseline legs of bench.py and scripts under scripts/ do.
+The reference tree is looked up at $PAINTER_REFERENCE, then at its default checkout location /root/reference, then in
+the staged byte-for-byte copy under oracle/_ref/ (scripts/stage_reference.py; git-ignored).  Nothing in the product
+path (painter_b200/*) imports this file: only tests/, the `--impl reference` / cpu_baseline legs of bench.py and
+scripts under scripts/ do.
 """
 import importlib
 import importlib.util
@@ -14,14 +14,16 @@ import types
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SHIMS = os.path.join(_HERE, "shims")
-_STAGED = os.path.join(os.path.dirname(_HERE), "baseline", "_ref")
+_STAGED = os.path.join(_HERE, "_ref")
+# default location of the baaivision/Painter checkout (overridden by $PAINTER_REFERENCE)
+DEFAULT_SOURCE = "/root/reference"
 
 
 def _find_root():
-    for cand in (os.environ.get("PAINTER_REFERENCE"), "/root/reference", _STAGED):
+    for cand in (os.environ.get("PAINTER_REFERENCE"), DEFAULT_SOURCE, _STAGED):
         if cand and os.path.isdir(os.path.join(cand, "Painter")):
             return cand
-    return "/root/reference"
+    return DEFAULT_SOURCE
 
 
 REF_ROOT = _find_root()

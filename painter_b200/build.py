@@ -1,4 +1,4 @@
-"""Build libpainter_b200.so in-tree with nvcc for sm_100a (no torch extension machinery).
+"""Build libpainter_b200.so in-tree with nvcc for sm_90a (H100) (no torch extension machinery).
 
     python -m painter_b200.build          # incremental
     python -m painter_b200.build --force
@@ -14,7 +14,7 @@ OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libpainter_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
 
@@ -54,7 +54,7 @@ def build(force=False, verbose=False):
             if r.returncode != 0:
                 raise RuntimeError("nvcc failed: " + " ".join(cmd))
     if jobs or not os.path.exists(LIB):
-        cmd = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             sys.stderr.write(r.stdout + r.stderr)

@@ -1,27 +1,43 @@
-// painter_b200 — persistent, warp-specialised tcgen05 GEMM for sm_100a.
+// painter_b200 — persistent, warp-specialised wgmma GEMM for sm_90a.
 //
-//   C[M,N] = A[M,K] . B[N,K]^T      bf16 operands, fp32 accumulation in TMEM
+//   C[M,N] = A[M,K] . B[N,K]^T      bf16 operands, fp32 accumulation in registers
 //
-// One CTA per SM, 256 threads:
-//   warps 0..3  epilogue       (tcgen05.ld 32x32b -> registers -> smem staging -> coalesced fused epilogue)
-//   warp 4      TMA producer   (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx)
-//   warp 5      MMA issuer     (one elected lane: tcgen05.mma 128 x BN x 16, commit -> mbarriers)
-//   warp 6      TMEM allocator (2 accumulator stages of BN fp32 columns)
-// (producer / MMA warps have the highest ids on purpose: the issue arbiter prefers higher warp ids, and a busy
-//  epilogue warp must never delay the MMA issue)
-// The accumulator is double-buffered in TMEM so the epilogue of tile i overlaps the MMAs of tile
-// i+1.  Operands may be K-major (row-major [rows,K]) or MN-major (row-major [K,rows]); the latter is
-// what the backward GEMMs (dgrad: B = W[out,in]; wgrad: A = dY[tokens,out], B = X[tokens,in]) need, so no
-// transposed copies of weights or activations are ever materialised.
+// One CTA per SM, 384 threads, 128 x BN output tiles (BN = 64 / 128 / 256), K-blocks of 64:
+//   warpgroup 0     TMA producer   (one thread: cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx);
+//                                  gives its registers up (setmaxnreg) to the math warpgroups
+//   warpgroups 1-2  math           (wgmma.mma_async 64 x BN x 16 from shared memory, 64 accumulator rows each;
+//                                  one wgmma group stays in flight while the previous ring slot is released),
+//                                  then the fused epilogue: accumulators -> smem staging tile (64 x 64 per
+//                                  warpgroup) -> coalesced epilogue chunks of 32 x 32 per warp
+// The producer runs up to `stages` K-blocks ahead, so the next tile's operands stream in during an epilogue.
+// Operands may be K-major (row-major [rows,K]) or MN-major (row-major [K,rows]); the latter is what the backward
+// GEMMs (dgrad: B = W[out,in]; wgrad: A = dY[tokens,out], B = X[tokens,in]) need, so no transposed copies of weights
+// or activations are ever materialised.  Weight-gradient GEMMs (zero-initialised fp32 output) run stream-K.
 //
 // Reference call sites replaced: every nn.Linear on the path (models_painter.py:60-61,76,87; timm Mlp
 // fc1/fc2 via :201; decoder_embed :327,423) and autograd's mm backward for them.
 #include "gemm_common.cuh"
+#include "wgmma.cuh"
 
 namespace pk {
 
+// One 64-deep K-block of one math warpgroup: acc[64 x BN] (+)= A[64 x 64] . B[64 x BN]^T (4 wgmma, K = 16 each).
+template <int BN, int TA, int TB>
+__device__ __forceinline__ void gemm_kblock(float (&acc)[BN / 2], uint32_t a_addr, uint32_t b_addr, bool first) {
+  const uint64_t da = TA ? make_wgmma_desc(a_addr, 8192, 1024) : make_wgmma_desc(a_addr, 16, 1024);
+  const uint64_t db = TB ? make_wgmma_desc(b_addr, 8192, 1024) : make_wgmma_desc(b_addr, 16, 1024);
+  constexpr uint32_t a_step = TA ? 2048u : 32u, b_step = TB ? 2048u : 32u;
+#pragma unroll
+  for (int k = 0; k < GEMM_BK / 16; ++k) {
+    const uint64_t a = wgmma_desc_add(da, k * a_step), b = wgmma_desc_add(db, k * b_step);
+    const uint32_t accf = (first && k == 0) ? 0u : 1u;
+    if constexpr (BN == 64) wgmma_m64n64k16<TA, TB>(acc, a, b, accf);
+    else if constexpr (BN == 128) wgmma_m64n128k16<TA, TB>(acc, a, b, accf);
+    else wgmma_m64n256k16<TA, TB>(acc, a, b, accf);
+  }
+}
 
-template <int KIND>
+template <int KIND, int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const GemmArgs g) {
@@ -30,59 +46,46 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const uint32_t base = (raw_base + 1023u) & ~1023u;
   uint8_t* smem_gen = smem_raw + (base - raw_base);
 
-  const int BN = g.BN;
+  constexpr uint32_t B_BYTES = static_cast<uint32_t>(BN) * 128u;
   const int stages = g.stages;
-  const uint32_t B_BYTES = static_cast<uint32_t>(BN) * 128u;
   const uint32_t sA = base;
   const uint32_t sB = base + stages * GEMM_A_BYTES;
-  const uint32_t bar_base = sB + stages * B_BYTES;
-  // barrier layout: full[stages], empty[stages], tfull[2], tempty[2], holder
+  const uint32_t sStg = sB + stages * B_BYTES;
+  const uint32_t bar_base = sStg + GEMM_STG_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (stages + s); };
-  auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * stages + s); };
-  auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * stages + 2 + s); };
-  const uint32_t holder = bar_base + 8u * (2 * stages + 4);
-  volatile uint32_t* holder_gen =
-      reinterpret_cast<volatile uint32_t*>(smem_gen + (holder - base));
-  float* stg_gen = reinterpret_cast<float*>(smem_gen + (bar_base - base) + 256);  // 4 x [32][STG_LD] fp32
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
   const int num_kb = (g.K + GEMM_BK - 1) / GEMM_BK;
   const int tiles_mn = g.num_m_tiles * g.num_n_tiles;
-  const int total_tiles = tiles_mn * g.splits;
-  const uint32_t tmem_cols = 2u * BN;
 
-  if (warp == 8 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-  }
-  if (warp == 9 && lane == 0) {
     for (int s = 0; s < stages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tfull_bar(s), 1);
-      mbar_init(tempty_bar(s), GEMM_EPI_WARPS);
+      mbar_init(empty_bar(s), 256);   // every math thread releases the slot after its wgmma retired
     }
     fence_barrier_init();
   }
-  if (warp == 10) tmem_alloc(holder, tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *holder_gen;
+  pdl_launch_dependents();   // programmatic dependent launch (host_common.h): the prologue above overlaps the
+  pdl_wait();                // previous kernel's tail; nothing before this line touches global memory
 
-  if (warp == 8) {
-    if (lane == 0) {
+  GemmSched sch;
+  sch.init(g, tiles_mn, num_kb, blockIdx.x, gridDim.x);
+  int mn, kb0, kb1;
+
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
       // ------------------------------ TMA producer ------------------------------
       uint32_t s = 0, ph = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int mn = tile % tiles_mn, split = tile / tiles_mn;
-        const int m_blk = mn % g.num_m_tiles, n_blk = mn / g.num_m_tiles;
-        const int kb0 = split * g.kb_per_split;
-        const int kb1 = min(num_kb, kb0 + g.kb_per_split);
+      while (sch.next(mn, kb0, kb1)) {
+        int m_blk, n_blk;
+        gemm_tile_coords(g, mn, m_blk, n_blk);
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(empty_bar(s), ph ^ 1u);
           mbar_expect_tx(full_bar(s), GEMM_A_BYTES + B_BYTES);
@@ -127,158 +130,161 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
     }
-  } else if (warp == 9) {
-    {
-      // ------------------------------- MMA issuer -------------------------------
-      // warp-uniform control flow (descriptors stay in uniform registers); one elected lane issues tcgen05
-      const uint32_t idesc = make_idesc_bf16(GEMM_BM, BN, g.transA != 0, g.transB != 0);
-      uint32_t s = 0, ph = 0, it = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-        const uint32_t as = it & 1u, aph = (it >> 1) & 1u;
-        mbar_wait(tempty_bar(as), aph ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * BN;
-        const int split = tile / tiles_mn;
-        const int kb0 = split * g.kb_per_split;
-        const int kb1 = min(num_kb, kb0 + g.kb_per_split);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(full_bar(s), ph);
-          tc_fence_after();
-          const uint32_t a_addr = sA + s * GEMM_A_BYTES;
-          const uint32_t b_addr = sB + s * B_BYTES;
-          const uint64_t a0 = g.transA ? make_sdesc(a_addr, 8192, 1024) : make_sdesc(a_addr, 16, 1024);
-          const uint64_t b0 = g.transB ? make_sdesc(b_addr, 8192, 1024) : make_sdesc(b_addr, 16, 1024);
-          const uint32_t a_step = g.transA ? 2048u : 32u, b_step = g.transB ? 2048u : 32u;
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < GEMM_BK / 16; ++k)
-              umma_ss(d_tmem, sdesc_add(a0, k * a_step), sdesc_add(b0, k * b_step), idesc,
-                      (kb != kb0 || k != 0) ? 1u : 0u);
-            umma_commit(empty_bar(s));
-          }
-          __syncwarp();
-          if (++s == static_cast<uint32_t>(stages)) {
-            s = 0;
-            ph ^= 1u;
-          }
-        }
-        if (elect_one()) umma_commit(tfull_bar(as));
-        __syncwarp();
-      }
-    }
-  } else if (warp < GEMM_EPI_WARPS) {
-    // --------------------------------- epilogue ---------------------------------
-    const int ew = warp & 3;   // TMEM lane quarter
-    const int eg = warp >> 2;  // column group: this warp owns the 64-column blocks with (c0 / 64) % 2 == eg
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      const int mn = tile % tiles_mn;
-      const int m_blk = mn % g.num_m_tiles, n_blk = mn / g.num_m_tiles;
-      const uint32_t as = it & 1u, aph = (it >> 1) & 1u;
-      mbar_wait(tfull_bar(as), aph);
-      tc_fence_after();
-      const int rloc = ew * 32 + lane;
-      const int row = m_blk * GEMM_BM + rloc;
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + as * BN;
-      if constexpr (KIND == EPI_HEAD || KIND == EPI_UNSHUF) {
-        // pixel-row tile (64 columns: handled by column group 0; group 1 only signals): rloc -> (b, y, x)
-        if (eg == 0) {
-        const int tx = m_blk % g.conv.tiles_x, r1 = m_blk / g.conv.tiles_x;
-        const int ty = r1 % g.conv.tiles_y, bi = r1 / g.conv.tiles_y;
-        const int y = ty * g.conv.TH + rloc / g.conv.TW, x = tx * g.conv.TW + rloc % g.conv.TW;
-        if constexpr (KIND == EPI_HEAD) {
-          float c[64];
-#pragma unroll
-          for (int c0 = 0; c0 < 64; c0 += 32) {
-            uint32_t v[32];
-            tmem_ld_x32(taddr + c0, v);
-            tmem_wait_ld();
-#pragma unroll
-            for (int j = 0; j < 32; ++j) c[c0 + j] = __uint_as_float(v[j]);
-          }
-          head_epilogue_row(g, bi, y, x, c);
-        } else {  // EPI_UNSHUF: token row m = (b, y/p, x/p), columns ((y%p)*p + x%p)*64 + c
-          const int p = g.epi.ps_p;
-          const size_t mtok = (static_cast<size_t>(bi) * (g.conv.H / p) + y / p) * (g.conv.W / p) + x / p;
-          __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(g.epi.out) + mtok * g.epi.ldc +
-                               ((y % p) * p + x % p) * 64 + n_blk * BN;
-          for (int c0 = 0; c0 < BN; c0 += 32) {
-            uint32_t v[32];
-            tmem_ld_x32(taddr + c0, v);
-            tmem_wait_ld();
-            float xv[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) xv[j] = __uint_as_float(v[j]);
-            store_bf16x32(dst + c0, xv);
-          }
-        }
-        }
-      } else {
-        float* stg = stg_gen + warp * (32 * STG_LD);
-        const int row0 = m_blk * GEMM_BM + ew * 32;
-        EpiAux auxA, auxB;   // explicit ping-pong (BN is a multiple of 64): keeps both in registers
-        if (eg * 64 < BN) gemm_epilogue_prefetch<KIND>(g.epi, row0, g.M, n_blk * BN + eg * 64, auxA);
-        for (int c0 = eg * 64; c0 < BN; c0 += 128) {
-          uint32_t v[32];
-          tmem_ld_x32(taddr + c0, v);
-          gemm_epilogue_prefetch<KIND>(g.epi, row0, g.M, n_blk * BN + c0 + 32, auxB);
-          tmem_wait_ld();
-          gemm_epilogue_chunk<KIND>(g.epi, stg, row0, g.M, n_blk * BN + c0, v, auxA);
-          tmem_ld_x32(taddr + c0 + 32, v);
-          if (c0 + 128 < BN) gemm_epilogue_prefetch<KIND>(g.epi, row0, g.M, n_blk * BN + c0 + 128, auxA);
-          tmem_wait_ld();
-          gemm_epilogue_chunk<KIND>(g.epi, stg, row0, g.M, n_blk * BN + c0 + 32, v, auxB);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(as));
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 10) tmem_dealloc(tmem_base, tmem_cols);
+  // ------------------------------------ math warpgroups ------------------------------------
+  setmaxnreg_inc<232>();
+  const int cw = wg - 1;                // accumulator rows [64 cw, 64 cw + 64) of the tile
+  const int wl = warp & 3;              // warp within the warpgroup
+  float* stg = reinterpret_cast<float*>(smem_gen + (sStg - base)) + cw * 64 * STG_LD;
+  const int frag_r = 16 * wl + (lane >> 2), frag_c = 2 * (lane & 3);
+  uint32_t s = 0, ph = 0;
+  float acc[BN / 2];
+  while (sch.next(mn, kb0, kb1)) {
+    int m_blk, n_blk;
+    gemm_tile_coords(g, mn, m_blk, n_blk);
+    int prev = -1;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(full_bar(s), ph);
+      const uint32_t a_addr = sA + s * GEMM_A_BYTES + cw * 8192;   // 64 K-major rows / one 64-wide MN group
+      const uint32_t b_addr = sB + s * B_BYTES;
+      wgmma_fence();
+      if (g.transA) {
+        if (g.transB) gemm_kblock<BN, 1, 1>(acc, a_addr, b_addr, kb == kb0);
+        else gemm_kblock<BN, 1, 0>(acc, a_addr, b_addr, kb == kb0);
+      } else {
+        if (g.transB) gemm_kblock<BN, 0, 1>(acc, a_addr, b_addr, kb == kb0);
+        else gemm_kblock<BN, 0, 0>(acc, a_addr, b_addr, kb == kb0);
+      }
+      wgmma_commit();
+      wgmma_fence_operands(acc);
+      wgmma_wait<1>();
+      wgmma_fence_operands(acc);
+      if (prev >= 0) mbar_arrive(empty_bar(prev));
+      prev = static_cast<int>(s);
+      if (++s == static_cast<uint32_t>(stages)) {
+        s = 0;
+        ph ^= 1u;
+      }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_operands(acc);
+    mbar_arrive(empty_bar(prev));
+
+    // --------------------------------- epilogue ---------------------------------
+#pragma unroll
+    for (int c0 = 0; c0 < BN; c0 += 64) {
+      named_bar_sync(1 + cw, 128);     // the previous chunk's readers are done with the staging tile
+#pragma unroll
+      for (int i = 0; i < BN / 2; i += 2) {
+        const int cb = 8 * (i / 4);
+        if (cb >= c0 && cb < c0 + 64) {
+          const int r = frag_r + 8 * ((i / 2) & 1);
+          *reinterpret_cast<float2*>(stg + r * STG_LD + cb - c0 + frag_c) = make_float2(acc[i], acc[i + 1]);
+        }
+      }
+      named_bar_sync(1 + cw, 128);
+      if constexpr (KIND == EPI_HEAD || KIND == EPI_UNSHUF) {
+        // pixel-row tile (BN = 64, one chunk): warps 0-1 of the warpgroup own one accumulator row per thread
+        if (wl < 2) {
+          const int rloc = cw * 64 + wl * 32 + lane;
+          const float* srow = stg + (wl * 32 + lane) * STG_LD;
+          const int tx = m_blk % g.conv.tiles_x, r1 = m_blk / g.conv.tiles_x;
+          const int ty = r1 % g.conv.tiles_y, bi = r1 / g.conv.tiles_y;
+          const int y = ty * g.conv.TH + rloc / g.conv.TW, x = tx * g.conv.TW + rloc % g.conv.TW;
+          float c[64];
+#pragma unroll
+          for (int q = 0; q < 16; ++q) {
+            const float4 v4 = reinterpret_cast<const float4*>(srow)[q];
+            c[4 * q] = v4.x; c[4 * q + 1] = v4.y; c[4 * q + 2] = v4.z; c[4 * q + 3] = v4.w;
+          }
+          if constexpr (KIND == EPI_HEAD) {
+            head_epilogue_row(g, bi, y, x, c);
+          } else {  // EPI_UNSHUF: token row m = (b, y/p, x/p), columns ((y%p)*p + x%p)*64 + c
+            const int p = g.epi.ps_p;
+            const size_t mtok = (static_cast<size_t>(bi) * (g.conv.H / p) + y / p) * (g.conv.W / p) + x / p;
+            __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(g.epi.out) + mtok * g.epi.ldc +
+                                 ((y % p) * p + x % p) * 64 + n_blk * BN;
+            store_bf16x32(dst, reinterpret_cast<const float(&)[32]>(c[0]));
+            store_bf16x32(dst + 32, reinterpret_cast<const float(&)[32]>(c[32]));
+          }
+        }
+      } else {
+        const int rb = (wl & 1) * 32, cb = (wl >> 1) * 32;
+        float* blk = stg + rb * STG_LD + cb;
+        const int row0 = m_blk * GEMM_BM + cw * 64 + rb;
+        const int col = n_blk * BN + c0 + cb;
+        EpiAux aux;
+        gemm_epilogue_prefetch<KIND>(g.epi, row0, g.M, col, aux);
+        uint32_t v[32];
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+          const float4 v4 = reinterpret_cast<const float4*>(blk + lane * STG_LD)[q];
+          v[4 * q] = __float_as_uint(v4.x); v[4 * q + 1] = __float_as_uint(v4.y);
+          v[4 * q + 2] = __float_as_uint(v4.z); v[4 * q + 3] = __float_as_uint(v4.w);
+        }
+        gemm_epilogue_chunk<KIND>(g.epi, blk, row0, g.M, col, v, aux);
+      }
+    }
+  }
 }
 
 int g_force_bn = 0;
 int g_force_splits = 0;
-int g_use_2cta = 1;  // 1 = CTA pairs (gemm2.cu) whenever the shape allows (default), 0 = 1-CTA kernel only
 
-int launch_gemm2(const void* A, const void* B, int lda, int ldb, GemmArgs& g, cudaStream_t st);
+static size_t gemm_smem_bytes(const GemmArgs& g) {
+  return 1024 + static_cast<size_t>(g.stages) * (GEMM_A_BYTES + g.BN * 128) + GEMM_STG_BYTES + 256;
+}
+
+// persistent CTAs a call runs: one per stream-K range, otherwise one per work item up to the SM count
+static int gemm_workers(const GemmArgs& g) {
+  const int num_kb = (g.K + GEMM_BK - 1) / GEMM_BK;
+  const long long tiles = static_cast<long long>(g.num_m_tiles) * g.num_n_tiles;
+  if (g.streamk_units > 0) return static_cast<int>((tiles * num_kb + g.streamk_units - 1) / g.streamk_units);
+  const long long items = tiles * g.splits;
+  return items < sm_count() ? static_cast<int>(items) : sm_count();
+}
+
+template <int KK, int BN>
+static cudaError_t launch_gemm_kernel(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmArgs& g,
+                                      cudaStream_t st) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_kernel<KK, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         227 * 1024);
+    if (e != cudaSuccess) return e;
+    attr_set = true;
+  }
+  return launch_pdl(gemm_bf16_kernel<KK, BN>, dim3(gemm_workers(g)), dim3(GEMM_THREADS), gemm_smem_bytes(g), st,
+                    tmA, tmB, g);
+}
+
+template <int KK>
+static cudaError_t launch_gemm_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmArgs& g,
+                                  cudaStream_t st) {
+  if (g.BN == 256) return launch_gemm_kernel<KK, 256>(tmA, tmB, g, st);
+  if (g.BN == 128) return launch_gemm_kernel<KK, 128>(tmA, tmB, g, st);
+  return launch_gemm_kernel<KK, 64>(tmA, tmB, g, st);
+}
 
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmArgs& g, cudaStream_t st,
                        const char* who) {
-  const size_t smem = 1024 + static_cast<size_t>(g.stages) * (GEMM_A_BYTES + g.BN * 128) + 256 +
-                      GEMM_EPI_WARPS * 32 * STG_LD * sizeof(float);
-  const int total = g.num_m_tiles * g.num_n_tiles * g.splits;
-  const int sms = sm_count();
-  const int grid = total < sms ? total : sms;
-#define PK_GEMM_CASE(KK)                                                                                       \
-  case KK: {                                                                                                   \
-    static bool attr_set = false;                                                                              \
-    if (!attr_set) {                                                                                           \
-      cudaError_t e = cudaFuncSetAttribute(gemm_bf16_kernel<KK>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
-                                           227 * 1024);                                                        \
-      PK_CHECK(e == cudaSuccess, "%s: cudaFuncSetAttribute: %s", who, cudaGetErrorString(e));                  \
-      attr_set = true;                                                                                         \
-    }                                                                                                          \
-    gemm_bf16_kernel<KK><<<grid, GEMM_THREADS, smem, st>>>(tmA, tmB, g);                                       \
-  } break;
+  PK_CHECK(gemm_smem_bytes(g) <= 227 * 1024 && g.stages >= 2, "%s: BN=%d does not fit shared memory", who, g.BN);
+  cudaError_t e = cudaSuccess;
   switch (g.epi.kind) {
-    PK_GEMM_CASE(PK_EPI_BF16)
-    PK_GEMM_CASE(PK_EPI_F32)
-    PK_GEMM_CASE(PK_EPI_GELU)
-    PK_GEMM_CASE(PK_EPI_RESID)
-    PK_GEMM_CASE(PK_EPI_DGELU)
-    PK_GEMM_CASE(PK_EPI_PIXSHUF)
-    PK_GEMM_CASE(EPI_HEAD)
-    PK_GEMM_CASE(EPI_UNSHUF)
+    case PK_EPI_BF16: e = launch_gemm_bn<PK_EPI_BF16>(tmA, tmB, g, st); break;
+    case PK_EPI_F32: e = launch_gemm_bn<PK_EPI_F32>(tmA, tmB, g, st); break;
+    case PK_EPI_GELU: e = launch_gemm_bn<PK_EPI_GELU>(tmA, tmB, g, st); break;
+    case PK_EPI_RESID: e = launch_gemm_bn<PK_EPI_RESID>(tmA, tmB, g, st); break;
+    case PK_EPI_DGELU: e = launch_gemm_bn<PK_EPI_DGELU>(tmA, tmB, g, st); break;
+    case PK_EPI_PIXSHUF: e = launch_gemm_bn<PK_EPI_PIXSHUF>(tmA, tmB, g, st); break;
+    case EPI_HEAD: e = launch_gemm_kernel<EPI_HEAD, 64>(tmA, tmB, g, st); break;
+    case EPI_UNSHUF: e = launch_gemm_kernel<EPI_UNSHUF, 64>(tmA, tmB, g, st); break;
     default:
       PK_CHECK(false, "%s: bad epilogue kind %d", who, g.epi.kind);
   }
-#undef PK_GEMM_CASE
+  PK_CHECK(e == cudaSuccess, "%s: launch: %s", who, cudaGetErrorString(e));
   PK_LAUNCH_CHECK(who);
   return 0;
 }
@@ -298,14 +304,11 @@ static bool conv_tile_geometry(int H, int W, int pixels, int* TW, int* TH) {
 // test hooks: force the N tile (64/128/256) / the split-K factor; 0 restores the heuristics
 extern "C" void pk_gemm_force_bn(int bn) { pk::g_force_bn = bn; }
 extern "C" void pk_gemm_force_splits(int s) { pk::g_force_splits = s; }
-extern "C" void pk_gemm_use_2cta(int on) { pk::g_use_2cta = on; }
 
 // Tiling / scheduling decisions of one pk_gemm_bf16 call (host only; also reachable through pk_gemm_plan for the
-// CPU-side schedule tests).  Returns the kernel arguments and which kernel (CTA pair or single CTA) runs them.
-static void plan_gemm(int M, int N, int K, int transA, int transB, const PkEpilogue* epi, pk::GemmArgs& gout,
-                      bool& two_cta) {
+// CPU-side schedule tests).
+static void plan_gemm(int M, int N, int K, int transA, int transB, const PkEpilogue* epi, pk::GemmArgs& g) {
   using namespace pk;
-  GemmArgs g;
   memset(&g, 0, sizeof(g));
   g.M = M;
   g.N = N;
@@ -316,76 +319,51 @@ static void plan_gemm(int M, int N, int K, int transA, int transB, const PkEpilo
   if (g.epi.alpha == 0.0f) g.epi.alpha = 1.0f;
   const int sms = sm_count();
   const int mt = (M + GEMM_BM - 1) / GEMM_BM;
+  const bool zero_init_f32 = epi->kind == PK_EPI_F32 && epi->accumulate == 2;
+  // 128 x 128 tiles where the shape allows.  BN = 256 (128 accumulator registers per math thread) exceeds the
+  // 168-register budget of a 384-thread CTA once the epilogue's registers are live and spills; it stays reachable
+  // through pk_gemm_force_bn only.
   int BN = 64;
-  const bool can_split = epi->kind == PK_EPI_F32 && epi->accumulate == 2;
-  if (can_split) {
-    // weight-gradient GEMMs (K = tokens): take the widest tile and fill the machine with split-K instead of
+  if (zero_init_f32) {
+    // weight-gradient GEMMs (K = tokens): take the wide tile and fill the machine with stream-K instead of
     // shrinking the tile
-    BN = N % 256 == 0 ? 256 : (N % 128 == 0 ? 128 : 64);
-  } else {
-    if (N % 256 == 0 && static_cast<long long>(mt) * (N / 256) >= sms) BN = 256;
-    else if (N % 128 == 0 && static_cast<long long>(mt) * (N / 128) >= sms / 2) BN = 128;
+    if (N % 128 == 0) BN = 128;
+  } else if (N % 128 == 0 && static_cast<long long>(mt) * (N / 128) >= sms / 2) {
+    BN = 128;
   }
   if (g_force_bn > 0 && N % g_force_bn == 0) BN = g_force_bn;
   g.BN = BN;
   g.stages = gemm_stages_for(GEMM_A_BYTES + BN * 128);
   g.num_m_tiles = mt;
   g.num_n_tiles = N / BN;
-  // split-K: only for plain fp32 outputs whose tile count cannot fill the machine (wgrad GEMMs);
-  // accumulate == 2 means "out is zero-initialised, add atomically".
   const int num_kb = (K + GEMM_BK - 1) / GEMM_BK;
   g.splits = 1;
-  if (epi->kind == PK_EPI_F32 && epi->accumulate == 2) {
-    int want = sms / (g.num_m_tiles * g.num_n_tiles);
-    if (want > 1) {
-      if (want > num_kb / 8) want = num_kb / 8 > 0 ? num_kb / 8 : 1;
-      g.splits = want;
+  g.kb_per_split = num_kb;
+  if (zero_init_f32) {
+    // zero-initialised fp32 output (weight gradients): stream-K.  The tiles_mn * num_kb k-block units are cut into
+    // one equal range per CTA; a tile that straddles ranges is finished with fp32 atomics.
+    const int tiles = g.num_m_tiles * g.num_n_tiles;
+    const long long units = static_cast<long long>(tiles) * num_kb;
+    if (g_force_splits > 0) {
+      const int want = g_force_splits < num_kb ? g_force_splits : num_kb;
+      g.kb_per_split = (num_kb + want - 1) / want;
+      g.splits = (num_kb + g.kb_per_split - 1) / g.kb_per_split;
+      if (g.splits == 1) g.epi.accumulate = 1;
+    } else if (tiles % sms == 0 || units < 4ll * sms) {
+      g.epi.accumulate = 1;   // already balanced (or too small to matter): plain data-parallel tiles
+    } else {
+      int per = static_cast<int>((units + sms - 1) / sms);
+      if (per < 4) per = 4;
+      g.streamk_units = per;
     }
-    if (g_force_splits > 0) g.splits = g_force_splits < num_kb ? g_force_splits : num_kb;
   }
-  g.kb_per_split = (num_kb + g.splits - 1) / g.splits;
-  g.splits = (num_kb + g.kb_per_split - 1) / g.kb_per_split;
-  if (g.splits == 1 && g.epi.kind == PK_EPI_F32 && g.epi.accumulate == 2) g.epi.accumulate = 1;
-
-  // CTA-pair kernel (256 x BN tiles): needs a pair-tile count that can feed 74 clusters
-  two_cta = g_use_2cta && (BN == 256 || BN == 128) && M >= 256;
-  if (two_cta) {
-    GemmArgs g2 = g;
-    g2.num_m_tiles = (M + 255) / 256;
-    g2.stages = gemm_stages_for(GEMM_A_BYTES + (BN / 2) * 128);
-    if (g2.epi.kind == PK_EPI_F32 && epi->accumulate == 2) {
-      // zero-initialised fp32 output (weight gradients): stream-K.  The tiles_mn * num_kb k-block units are cut
-      // into one equal range per cluster; a tile that straddles ranges is finished with fp32 atomics.
-      g2.epi.accumulate = 2;
-      g2.splits = 1;
-      g2.kb_per_split = num_kb;
-      const int clusters = sms / 2;
-      const int tiles2 = g2.num_m_tiles * g2.num_n_tiles;
-      const long long units = static_cast<long long>(tiles2) * num_kb;
-      if (g_force_splits > 0) {
-        const int want = g_force_splits < num_kb ? g_force_splits : num_kb;
-        g2.kb_per_split = (num_kb + want - 1) / want;
-        g2.splits = (num_kb + g2.kb_per_split - 1) / g2.kb_per_split;
-        if (g2.splits == 1) g2.epi.accumulate = 1;
-      } else if (tiles2 % clusters == 0 || units < 4ll * clusters) {
-        g2.epi.accumulate = 1;   // already balanced (or too small to matter): plain data-parallel tiles
-      } else {
-        int per = static_cast<int>((units + clusters - 1) / clusters);
-        if (per < 4) per = 4;
-        g2.streamk_units = per;
-      }
-    }
-    // rasterisation: keep B L2-resident when it fits, otherwise sweep the columns inside groups of 8 row blocks
-    // (stream-K calls with a large B keep the row-fastest order: measured 1006 vs 918 TF/s on the decoder wgrad)
-    g2.group_m = (static_cast<long long>(N) * K * 2 <= (40ll << 20)) ? 1 : (g2.streamk_units > 0 ? 0 : 8);
-    gout = g2;
-    return;
-  }
-  gout = g;
+  // rasterisation: keep B L2-resident when it fits, otherwise sweep the columns inside groups of 8 row blocks
+  // (stream-K calls keep the row-fastest order)
+  g.group_m = (static_cast<long long>(N) * K * 2 <= (40ll << 20)) ? 1 : (g.streamk_units > 0 ? 0 : 8);
 }
 
 // Host-side views of the scheduler (no device work): the plan of a call, and the (row block, column block, k-block
-// range) items one cluster / CTA walks - the same GemmSched / gemm_tile_coords code the kernels run.
+// range) items one CTA walks - the same GemmSched / gemm_tile_coords code the kernel runs.
 extern "C" int pk_gemm_plan(int M, int N, int K, int kind, int accumulate, int* out9) {
   using namespace pk;
   PK_CHECK(out9 && M > 0 && N > 0 && K > 0 && N % 64 == 0, "pk_gemm_plan: bad arguments");
@@ -394,20 +372,9 @@ extern "C" int pk_gemm_plan(int M, int N, int K, int kind, int accumulate, int* 
   e.kind = kind;
   e.accumulate = accumulate;
   GemmArgs g;
-  bool two = false;
-  plan_gemm(M, N, K, 0, 0, &e, g, two);
-  const int num_kb = (K + GEMM_BK - 1) / GEMM_BK;
-  const int tiles = g.num_m_tiles * g.num_n_tiles;
-  int workers;
-  if (two) {
-    workers = sm_count() / 2;
-    if (g.streamk_units > 0) workers = (tiles * num_kb + g.streamk_units - 1) / g.streamk_units;
-    else if (workers > tiles * g.splits) workers = tiles * g.splits;
-  } else {
-    workers = sm_count() < tiles * g.splits ? sm_count() : tiles * g.splits;
-  }
-  const int vals[9] = {two ? 1 : 0, g.BN, g.num_m_tiles, g.num_n_tiles, g.splits, g.kb_per_split, g.streamk_units,
-                       g.group_m, workers};
+  plan_gemm(M, N, K, 0, 0, &e, g);
+  const int vals[9] = {0, g.BN, g.num_m_tiles, g.num_n_tiles, g.splits, g.kb_per_split, g.streamk_units,
+                       g.group_m, gemm_workers(g)};
   for (int i = 0; i < 9; ++i) out9[i] = vals[i];
   return 0;
 }
@@ -415,36 +382,22 @@ extern "C" int pk_gemm_plan(int M, int N, int K, int kind, int accumulate, int* 
 extern "C" int pk_gemm_plan_walk(int M, int N, int K, int kind, int accumulate, int worker, int* out4, int max_items) {
   using namespace pk;
   PK_CHECK(out4 && max_items > 0, "pk_gemm_plan_walk: bad arguments");
-  int plan[9];
-  if (pk_gemm_plan(M, N, K, kind, accumulate, plan)) return 2;
+  PK_CHECK(M > 0 && N > 0 && K > 0 && N % 64 == 0, "pk_gemm_plan_walk: bad arguments");
   PkEpilogue e;
   memset(&e, 0, sizeof(e));
   e.kind = kind;
   e.accumulate = accumulate;
   GemmArgs g;
-  bool two = false;
-  plan_gemm(M, N, K, 0, 0, &e, g, two);
+  plan_gemm(M, N, K, 0, 0, &e, g);
   const int num_kb = (K + GEMM_BK - 1) / GEMM_BK;
-  const int tiles = g.num_m_tiles * g.num_n_tiles;
-  int n = 0;
-  if (two) {
-    GemmSched sch;
-    sch.init(g, tiles, num_kb, worker, plan[8]);
-    int mn, kb0, kb1;
-    while (sch.next(mn, kb0, kb1) && n < max_items) {
-      int mb, nb;
-      gemm_tile_coords(g, mn, mb, nb);
-      out4[4 * n] = mb; out4[4 * n + 1] = nb; out4[4 * n + 2] = kb0; out4[4 * n + 3] = kb1;
-      ++n;
-    }
-  } else {
-    for (int tile = worker; tile < tiles * g.splits && n < max_items; tile += plan[8]) {
-      const int mn = tile % tiles, split = tile / tiles;
-      const int kb0 = split * g.kb_per_split;
-      const int kb1 = num_kb < kb0 + g.kb_per_split ? num_kb : kb0 + g.kb_per_split;
-      out4[4 * n] = mn % g.num_m_tiles; out4[4 * n + 1] = mn / g.num_m_tiles; out4[4 * n + 2] = kb0; out4[4 * n + 3] = kb1;
-      ++n;
-    }
+  GemmSched sch;
+  sch.init(g, g.num_m_tiles * g.num_n_tiles, num_kb, worker, gemm_workers(g));
+  int n = 0, mn, kb0, kb1;
+  while (n < max_items && sch.next(mn, kb0, kb1)) {
+    int mb, nb;
+    gemm_tile_coords(g, mn, mb, nb);
+    out4[4 * n] = mb; out4[4 * n + 1] = nb; out4[4 * n + 2] = kb0; out4[4 * n + 3] = kb1;
+    ++n;
   }
   return -n;   // number of items, negated (0 and positive values are the usual status codes)
 }
@@ -473,16 +426,14 @@ extern "C" int pk_gemm_bf16(const void* A, const void* B, int M, int N, int K, i
              "pk_gemm_bf16: bad pixel-shuffle geometry");
 
   GemmArgs g;
-  bool two_cta = false;
-  plan_gemm(M, N, K, transA, transB, epi, g, two_cta);
-  if (two_cta) return launch_gemm2(A, B, lda, ldb, g, static_cast<cudaStream_t>(stream));
+  plan_gemm(M, N, K, transA, transB, epi, g);
 
   CUtensorMap tmA, tmB;
   {
     uint64_t dims[2], strides[1];
     uint32_t box[2];
     if (!g.transA) {
-      dims[0] = K; dims[1] = M; box[0] = 64; box[1] = 128;
+      dims[0] = K; dims[1] = M; box[0] = 64; box[1] = GEMM_BM;
     } else {
       dims[0] = M; dims[1] = K; box[0] = 64; box[1] = 64;
     }

@@ -1,5 +1,5 @@
-// painter_b200 — pieces shared by the 1-CTA (gemm.cu) and 2-CTA (gemm2.cu) tcgen05 GEMM kernels:
-// argument structs, the fused epilogues and the decoder-head epilogue.
+// painter_b200 — pieces of the wgmma GEMM (gemm.cu) shared with its host-side planner: argument structs, the
+// work scheduler, the fused epilogues and the decoder-head epilogue.
 #pragma once
 #include <string.h>
 
@@ -12,8 +12,9 @@ namespace pk {
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;
 constexpr int GEMM_A_BYTES = GEMM_BM * GEMM_BK * 2;  // 16 KiB
-constexpr int GEMM_THREADS = 352;   // 8 epilogue warps + TMA warp + MMA warp + TMEM-allocator warp
-constexpr int GEMM_EPI_WARPS = 8;
+constexpr int GEMM_THREADS = 384;   // TMA producer warpgroup + two math warpgroups (64 accumulator rows each)
+constexpr int STG_LD = 68;          // floats per row of a math warpgroup's 64 x 64 epilogue staging tile
+constexpr int GEMM_STG_BYTES = 2 * 64 * STG_LD * 4;
 
 // internal epilogue kinds (beyond the public PK_EPI_*)
 constexpr int EPI_HEAD = 100;    // decoder head fused behind the 3x3 conv (LN2D + GELU + 1x1 conv + loss)
@@ -39,9 +40,9 @@ struct HeadArgs {
   int slot;                 // which copy of the head parameters in constant memory this launch reads
 };
 
-// operand ring depth that fits beside the 8 epilogue staging tiles
+// operand ring depth that fits beside the two epilogue staging tiles
 __host__ inline int gemm_stages_for(int stage_bytes) {
-  const int budget = 227 * 1024 - 1024 - 256 - GEMM_EPI_WARPS * 32 * 36 * 4 - GEMM_EPI_WARPS * 128 * 4;
+  const int budget = 227 * 1024 - 1024 - 256 - GEMM_STG_BYTES;
   int st = budget / stage_bytes;
   return st > 8 ? 8 : st;
 }
@@ -53,19 +54,19 @@ struct GemmArgs {
   int transA, transB;
   int num_m_tiles, num_n_tiles;
   int splits, kb_per_split;  // split-K (epilogue accumulates with fp32 atomics when splits > 1)
-  int streamk_units;         // > 0: stream-K (2-CTA kernel): every cluster owns this many consecutive
-                             // (tile, k-block) units; partial tiles are added with fp32 atomics
+  int streamk_units;         // > 0: stream-K: every CTA owns this many consecutive (tile, k-block) units;
+                             // partial tiles are added with fp32 atomics
   int group_m;               // tile rasterisation: groups of group_m row blocks, the column blocks of a group
-                             // consecutive (0 = row blocks fastest, the 1-CTA kernel's order)
+                             // consecutive (0 = row blocks fastest)
   PkEpilogue epi;
   ConvArgs conv;
   HeadArgs head;
 };
 
-// Work iterator shared by the producer / MMA / epilogue roles of the persistent kernels: each role walks the same
-// sequence of (output tile, k-block range) items.  Classic mode: item = (tile, split) strided over the clusters;
-// stream-K mode: the tiles_mn * num_kb k-block units are cut into equal consecutive ranges, one per cluster, so the
-// machine is full whatever the tile count (weight-gradient GEMMs have 16..64 tiles for 74 clusters).
+// Work iterator shared by the producer and math roles of the persistent kernel: each role walks the same sequence
+// of (output tile, k-block range) items.  Classic mode: item = (tile, split) strided over the CTAs; stream-K mode:
+// the tiles_mn * num_kb k-block units are cut into equal consecutive ranges, one per CTA, so the machine is full
+// whatever the tile count (weight-gradient GEMMs have 32..128 tiles for 132 SMs).
 struct GemmSched {
   int tiles_mn, num_kb, kbps, total, ncl, cur, end;
   bool sk;
@@ -104,11 +105,10 @@ struct GemmSched {
   }
 };
 
-// Linear tile index -> (row block, column block).  Concurrent clusters should share operand blocks so that each is
+// Linear tile index -> (row block, column block).  Concurrent CTAs should share operand blocks so that each is
 // fetched from HBM once and from L2 otherwise: with group_m = 1 the column blocks of one row block are adjacent
-// (A read once; right whenever B - weights, <= 40 MB - stays L2-resident: the N = 1024 GEMMs with K = 4096 read 2.3x
-// their algorithmic bytes with row blocks fastest); larger groups bound the B re-reads when B does not fit
-// (decoder_embed: 134 MB of weights).
+// (A read once; right whenever B - weights, <= 40 MB - stays resident in the 50 MB L2); larger groups bound the B
+// re-reads when B does not fit (decoder_embed: 134 MB of weights).
 __host__ __device__ __forceinline__ void gemm_tile_coords(const GemmArgs& g, int mn, int& m_blk, int& n_blk) {
   if (g.group_m <= 0) {
     m_blk = mn % g.num_m_tiles;
@@ -214,11 +214,11 @@ __device__ __forceinline__ void store_bf16x32(__nv_bfloat16* dst, const float (&
   }
 }
 
-// Generic epilogue for one 32-row x 32-column accumulator chunk of one epilogue warp.
-// Phase 1 (thread = accumulator row): alpha, bias, per-sample row scale -> private smem staging tile.
+// Generic epilogue for one 32-row x 32-column accumulator chunk of one warp.  `stg` is the warp's 32 x 32 block of
+// its warpgroup's staging tile (row stride STG_LD floats: 16-byte aligned, conflict-free for float4 quarter-warps).
+// Phase 1 (thread = accumulator row): alpha, bias, per-sample row scale -> back into the staging block.
 // Phase 2 (lane = 4 consecutive columns, 8 lanes per row, 4 rows per instruction): every global access of the
 // warp covers whole contiguous row segments (128 B fp32 / 64 B bf16) instead of 32 scattered rows.
-constexpr int STG_LD = 36;  // floats per staged row: 16-byte aligned, conflict-free for float4 quarter-warps
 
 __device__ __forceinline__ uint2 pack4_bf16(const float4& v) {
   uint2 u;
@@ -232,8 +232,7 @@ __device__ __forceinline__ float4 unpack4_bf16(const uint2& u) {
 }
 
 // Global reads a chunk's epilogue needs (residual / saved pre-activation / accumulate-into output), in the
-// coalesced phase-2 layout.  Issued one chunk AHEAD of their use so that their latency overlaps the TMEM load,
-// the staging pass and the previous chunk's stores.
+// coalesced phase-2 layout.
 struct EpiAux {
   float4 f[8];
   uint2 h[8];
@@ -272,12 +271,9 @@ __device__ __forceinline__ void gemm_epilogue_prefetch(const PkEpilogue& e, int 
   }
 }
 
-// bias_s: optional shared-memory copy of the 32 bias values of this chunk (staged by the caller at tile start, so
-// that the chunk does not start with a global-memory round trip); nullptr = read e.bias through the read-only cache.
 template <int KIND>
 __device__ __forceinline__ void gemm_epilogue_chunk(const PkEpilogue& e, float* stg, int row0, int M, int col,
-                                                    const uint32_t (&v)[32], const EpiAux& aux,
-                                                    const float* bias_s = nullptr) {
+                                                    const uint32_t (&v)[32], const EpiAux& aux) {
   const int lane = threadIdx.x & 31;
   const int rsub = lane >> 3, c4 = (lane & 7) * 4;
   const int cc = col + c4;
@@ -290,11 +286,11 @@ __device__ __forceinline__ void gemm_epilogue_chunk(const PkEpilogue& e, float* 
     if (KIND == PK_EPI_RESID && e.rowscale != nullptr && row < M) sc *= __ldg(e.rowscale + row / e.rows_per_group);
     float4* srow = reinterpret_cast<float4*>(stg + lane * STG_LD);
     if (e.bias != nullptr) {
-      const float4* b4 = reinterpret_cast<const float4*>(bias_s != nullptr ? bias_s : e.bias + col);
+      const float4* b4 = reinterpret_cast<const float4*>(e.bias + col);
       const float bsc = KIND == PK_EPI_RESID ? sc / e.alpha : 1.0f;  // rowscale also multiplies the bias
 #pragma unroll
       for (int q = 0; q < 8; ++q) {
-        const float4 b = bias_s != nullptr ? b4[q] : __ldg(b4 + q);
+        const float4 b = __ldg(b4 + q);
         srow[q] = make_float4(fmaf(__uint_as_float(v[q * 4 + 0]), sc, b.x * bsc),
                               fmaf(__uint_as_float(v[q * 4 + 1]), sc, b.y * bsc),
                               fmaf(__uint_as_float(v[q * 4 + 2]), sc, b.z * bsc),

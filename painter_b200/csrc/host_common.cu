@@ -20,7 +20,8 @@ void set_error(const char* fmt, ...) {
 
 static std::atomic<int> g_sm_budget{0};
 
-// SM count of the CURRENT device (cached per device ordinal), capped by pk_set_sm_budget and kept even (CTA pairs).
+// SM count of the CURRENT device (cached per device ordinal), capped by pk_set_sm_budget.  Without a device (host-only
+// schedule queries) the H100 SXM's 132 SMs.
 int sm_count() {
   static std::atomic<int> cache[64];
   int dev = 0;
@@ -28,12 +29,12 @@ int sm_count() {
   int n = (dev >= 0 && dev < 64) ? cache[dev].load(std::memory_order_relaxed) : 0;
   if (n == 0) {
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
     if (dev >= 0 && dev < 64) cache[dev].store(n, std::memory_order_relaxed);
   }
   const int b = g_sm_budget.load(std::memory_order_relaxed);
-  if (b > 0 && b < n) n = b & ~1;
-  return n < 2 ? 2 : n;
+  if (b > 0 && b < n) n = b;
+  return n < 1 ? 1 : n;
 }
 
 static std::atomic<int> g_pdl{-1};

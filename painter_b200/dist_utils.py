@@ -35,7 +35,7 @@ class GradSync:
     all-reduce(mean) of that range is issued asynchronously (NCCL runs it on its own stream after the producing
     kernels, over NVLink / NVSwitch), so communication overlaps the rest of backward with no copy into separate
     buckets and a handful of large collectives per step.  The last stage waits for all of them.  While collectives
-    are in flight the persistent tcgen05 GEMMs size their grids for `148 - sm_reserve` SMs, so that a NCCL kernel
+    are in flight the persistent GEMM sizes its grid for `132 - sm_reserve` SMs, so that a NCCL kernel
     holding a few SMs never pushes statically scheduled tiles into a second wave.
 
     Semantics = DDP: parameters are broadcast from rank 0 at construction, gradients are averaged over ranks

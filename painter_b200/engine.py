@@ -167,9 +167,8 @@ class BlockFn(torch.autograd.Function):
         wfc1, wfc2 = bf16_weight(fc1_w), bf16_weight(fc2_w)
         th, tw = bf16_table(rel_h), bf16_table(rel_w)
         # ops.attn_fwd(save_rel=True) / attn_bwd(rel=...) can keep every query's bias rows for the backward (the dQ
-        # kernel then loads them instead of recomputing two small MMAs and the Toeplitz gathers).  Measured on the
-        # B200 at batch 8: dQ kernel 0.325 -> 0.320 ms, forward 0.161 -> 0.164 ms - neutral - for 72 MB of extra saved
-        # activations per block application, so the module does not use it.
+        # kernel then loads them instead of recomputing them).  That costs 72 MB of extra saved activations per block
+        # application at batch 8 and saves one small kernel, so the module does not use it.
         save_rel = False
         relh = relw = x.new_empty(0)
         if ws > 0:

@@ -1,11 +1,11 @@
-"""B200-native drop-in for the reference `Painter` module (Painter/models_painter.py:238-487).
+"""H100-native drop-in for the reference `Painter` module (Painter/models_painter.py:238-487).
 
 Same constructor arguments, same `forward(imgs, tgts, bool_masked_pos=None, valid=None)` ->
 `(loss, patchify(pred), bool_masked_pos)`, same attributes (`patch_size`, `patch_embed.num_patches`, `blocks`,
 `pos_embed`, `no_weight_decay()`, `patchify/unpatchify`) and IDENTICAL state-dict keys/shapes, so
 `painter_vit_large.pth` / MAE checkpoints load and `engine_train.train_one_epoch` runs unchanged.  The
 `nn.Linear / nn.LayerNorm / nn.Conv2d` children are parameter holders only: their `forward` is never called —
-all arithmetic goes through painter_b200.engine (hand-written sm_100a kernels).  There is no CPU path.
+all arithmetic goes through painter_b200.engine (hand-written sm_90a kernels).  There is no CPU path.
 """
 from functools import partial
 
@@ -248,7 +248,7 @@ class Painter(nn.Module):
 
     def _run(self, imgs, tgts, bool_masked_pos, valid, seg_type=None, merge_between_batch=-1):
         if not imgs.is_cuda:
-            raise RuntimeError("painter_b200 runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("painter_b200 runs on CUDA (sm_90a) only; there is no CPU fallback")
         if valid is None:
             raise ValueError("valid must be given (the reference forward_loss multiplies by it, models_painter.py:450)")
         p = self.patch_size

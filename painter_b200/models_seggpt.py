@@ -1,4 +1,4 @@
-"""B200-native drop-in for the reference `SegGPT` module (SegGPT/SegGPT_inference/models_seggpt.py:241-494):
+"""H100-native drop-in for the reference `SegGPT` module (SegGPT/SegGPT_inference/models_seggpt.py:241-494):
 Painter plus seg-type tokens (:285-286,:414-420), the multi-prompt feature ensemble (:220-231,:425-429) and the
 loss without the ignore test (:448-469).  `forward(imgs, tgts, bool_masked_pos, valid, seg_type,
 merge_between_batch)` keeps the positional order used by seggpt_engine.run_one_image (:47)."""

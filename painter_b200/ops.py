@@ -31,7 +31,7 @@ def _req(t, dtype, name):
 
 def gemm(a, b, *, trans_a=False, trans_b=False, kind=EPI_BF16, out=None, out2=None, bias=None,
          aux=None, rowscale=None, rows_per_group=0, alpha=1.0, accumulate=False, pixshuf=None):
-    """C[M,N] = A[M,K] . B[N,K]^T on tcgen05 (bf16 in, fp32 accumulate).
+    """C[M,N] = A[M,K] . B[N,K]^T on the tensor cores (wgmma; bf16 in, fp32 accumulate).
 
     a: [M,K] (or [K,M] when trans_a);  b: [N,K] (or [K,N] when trans_b); last dim contiguous.
     pixshuf = (h, w, p, c, out_tensor[B, h*p, w*p, c]) for EPI_PIXSHUF.

@@ -1,4 +1,4 @@
-"""B200-side mirror of the Painter task-inference `run_one_image` functions (SURVEY §8 f.2), e.g.
+"""GPU-side mirror of the Painter task-inference `run_one_image` functions (SURVEY §8 f.2), e.g.
 Painter/eval/ade20k_semantic/painter_inference_segm.py:67-93: same arguments, same PNG on disk, with the
 nhwc->nchw conversion, the forward (CUDA-graph replay), unpatchify + bottom half + de-normalisation + clip and the
 bilinear resize to the source size on the GPU; only the final uint8 image crosses back to the host."""

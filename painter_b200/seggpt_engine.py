@@ -1,4 +1,4 @@
-"""B200-side mirror of SegGPT/SegGPT_inference/seggpt_engine.py (SURVEY §8 f.2): the same three entry points
+"""GPU-side mirror of SegGPT/SegGPT_inference/seggpt_engine.py (SURVEY §8 f.2): the same three entry points
 
     run_one_image(img, tgt, model, device)                                   seggpt_engine.py:26-53
     inference_image(model, device, img_path, img2_paths, tgt2_paths, out_path)       :56-103

@@ -1,4 +1,4 @@
-"""GPU bring-up check of the tcgen05 GEMM (runs every case in a subprocess so that a trapped kernel
+"""GPU bring-up check of the wgmma GEMM (runs every case in a subprocess so that a trapped kernel
 does not poison the rest).  Usage on the GPU box:  python scripts/gpu_check_gemm.py [--out file]"""
 import json
 import os
@@ -62,7 +62,6 @@ def run_case(name, M, N, K, ta, tb, kind, bn):
     b_in = b.t().contiguous() if tb else b
     ref = a.float() @ b.float().t()
     _lib.lib().pk_gemm_force_bn(bn)
-    _lib.lib().pk_gemm_use_2cta(int(os.environ.get("PK_2CTA", "0")))
     _lib.lib().pk_gemm_force_splits(int(os.environ.get("PK_FORCE_SPLITS", "0")))   # 0 = library heuristic
     bias = torch.randn(N, device=dev)
     kw = {}

@@ -1,14 +1,14 @@
 #!/usr/bin/env python
-"""Stage the UNMODIFIED reference (baaivision/Painter) into the git-ignored `baseline/_ref/` so that it travels to
-the GPU box with the gpurun snapshot (like the built .so files do) and can be executed there as the live oracle /
-reference arm:
+"""Stage the UNMODIFIED reference (baaivision/Painter) into the git-ignored `oracle/_ref/` so that a copy of the
+tree (like the built .so files) carries it to a GPU machine that has no checkout of the reference, where it is
+executed as the live oracle / reference arm:
 
-    python scripts/stage_reference.py            # copies from /root/reference (or $PAINTER_REFERENCE)
+    python scripts/stage_reference.py            # copies from $PAINTER_REFERENCE, else /root/reference
 
-The reference is pure Python with no setup.py, so `pip install --target baseline/_ref /root/reference` has nothing to
+The reference is pure Python with no setup.py, so `pip install --target oracle/_ref <reference>` has nothing to
 build (recorded in DESIGN.md); this script is the install step.  Only the files of the hot path, its two engines,
 the runtime utilities they import, the data pipeline used by the parity tests and the SegGPT example images are
-copied, byte for byte; nothing under baseline/_ref is tracked by git or imported by the product path.
+copied, byte for byte; nothing under oracle/_ref is tracked by git or imported by the product path.
 """
 import filecmp
 import os
@@ -16,7 +16,7 @@ import shutil
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-DST = os.path.join(ROOT, "baseline", "_ref")
+DST = os.path.join(ROOT, "oracle", "_ref")
 
 FILES = [
     "LICENSE",
@@ -36,8 +36,13 @@ FILES = [
 ]
 
 
+def source_root():
+    """Where the reference checkout is read from: $PAINTER_REFERENCE, else its default location."""
+    return os.environ.get("PAINTER_REFERENCE") or "/root/reference"
+
+
 def stage(src_root=None, verbose=True):
-    src_root = src_root or os.environ.get("PAINTER_REFERENCE", "/root/reference")
+    src_root = src_root or source_root()
     if not os.path.isdir(os.path.join(src_root, "Painter")):
         raise RuntimeError(f"reference tree not found at {src_root}")
     n = 0

@@ -1,7 +1,7 @@
 """Warm kernel timeline of the training step (torch.profiler / CUPTI): per-kernel totals inside real steps and the
 idle time between kernels on the compute stream.  Unlike the ncu launch list (cold caches, serialised replays) these
 are the durations the step actually sees.
-Usage (GPU box): python scripts/step_timeline.py [steps] > profiles/rNN_step_timeline.txt"""
+Usage (on the GPU machine): python scripts/step_timeline.py [steps] > step_timeline.txt"""
 import collections
 import os
 import sys

@@ -9,8 +9,23 @@ from oracle.synth import synth_inputs, synth_state_dict
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
+def _merge(dst, src):
+    for k, v in src.items():
+        if isinstance(v, dict) and isinstance(dst.get(k), dict):
+            _merge(dst[k], v)
+        else:
+            dst[k] = v
+
+
 def load_golden(name):
-    return torch.load(os.path.join(GOLDEN, name), weights_only=False)
+    """A golden file <stem>.pt, merged with its parts <stem>.part<i>.pt (nested dicts split so that every stored file
+    stays below 1 MB)."""
+    stem = name[:-3]
+    gold = torch.load(os.path.join(GOLDEN, name), weights_only=False)
+    parts = sorted(f for f in os.listdir(GOLDEN) if f.startswith(stem + ".part") and f.endswith(".pt"))
+    for f in parts:
+        _merge(gold, torch.load(os.path.join(GOLDEN, f), weights_only=False))
+    return gold
 
 
 def build_model(cfg: po.PainterConfig, seed, device="cuda", precision="bf16"):

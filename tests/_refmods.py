@@ -1,6 +1,9 @@
-"""TEST INFRASTRUCTURE: the UNMODIFIED reference modules (oracle/ref_loader.py: /root/reference here, the staged
-byte-for-byte copy baseline/_ref on the GPU box) loaded with the same synthetic weights as the painter_b200 module.
+"""TEST INFRASTRUCTURE: the UNMODIFIED reference modules (oracle/ref_loader.py: a checkout of the reference, or the
+staged byte-for-byte copy under oracle/_ref) loaded with the same synthetic weights as the painter_b200 module.
 """
+import json
+import os
+import tempfile
 from contextlib import contextmanager
 from functools import partial
 
@@ -9,6 +12,20 @@ import torch
 from oracle import painter_oracle as po
 from oracle import ref_loader
 from oracle.synth import synth_state_dict
+
+
+def record_parity(name, payload):
+    """Add one entry to the JSON parity report ($PK_PARITY_REPORT, default painter_parity.json in the temporary
+    directory): the measured error ratios of the tests against the live reference, kept for inspection."""
+    path = os.environ.get("PK_PARITY_REPORT") or os.path.join(tempfile.gettempdir(), "painter_parity.json")
+    try:
+        with open(path) as f:
+            allr = json.load(f)
+    except (OSError, ValueError):
+        allr = {}
+    allr[name] = payload
+    with open(path, "w") as f:
+        json.dump(allr, f, indent=1, sort_keys=True)
 
 
 def have_reference():

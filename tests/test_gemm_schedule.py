@@ -1,5 +1,5 @@
 """Host logic of the GEMM scheduler (no GPU): for every shape the engine issues, the work items of all workers
-(persistent clusters / CTAs) must tile the (row block, column block, k-block) space exactly once - classic
+(persistent CTAs) must tile the (row block, column block, k-block) space exactly once - classic
 split-K, stream-K and the grouped rasterisation all go through the same code the kernels execute
 (gemm_common.cuh: GemmSched, gemm_tile_coords; exported on the host as pk_gemm_plan / pk_gemm_plan_walk)."""
 import ctypes
@@ -52,14 +52,14 @@ def test_every_k_block_of_every_tile_is_covered_exactly_once(M, N, K, kind, acc)
             assert 0 <= mb < p["mt"] and 0 <= nb < p["nt"] and 0 <= k0 < k1 <= num_kb
             cover[mb, nb, k0:k1] += 1
     assert (cover == 1).all(), f"coverage min {cover.min()} max {cover.max()} for plan {p}"
-    if p["sk_units"] > 0:   # stream-K: every cluster but the last carries the same number of k-blocks
-        assert p["pair"] and acc == 2 and max(loads) == p["sk_units"] and min(loads[:-1]) == p["sk_units"]
+    if p["sk_units"] > 0:   # stream-K: every CTA but the last carries the same number of k-blocks
+        assert acc == 2 and max(loads) == p["sk_units"] and min(loads[:-1]) == p["sk_units"]
 
 
 def test_weight_gradient_shapes_take_stream_k_and_small_n_takes_column_fastest_raster():
     p = _plan(4096, 1024, 12544, EPI_F32, 2)
-    assert p["pair"] == 1 and p["sk_units"] > 0 and p["workers"] <= 74
+    assert p["sk_units"] > 0 and p["workers"] <= 132
     q = _plan(12544, 1024, 4096, EPI_RESID, 0)        # weights (8 MB) stay L2-resident: column blocks adjacent
-    assert q["pair"] == 1 and q["group_m"] == 1 and q["sk_units"] == 0
+    assert q["group_m"] == 1 and q["sk_units"] == 0
     d = _plan(12544, 16384, 4096, EPI_PIXSHUF, 0)     # 134 MB of weights: groups of 8 row blocks
     assert d["group_m"] == 8

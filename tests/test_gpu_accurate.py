@@ -8,7 +8,7 @@ from oracle import painter_oracle as po
 from oracle.synth import synth_inputs
 
 from _common import build_model, load_golden, rel_max
-from _refmods import build_reference, have_reference, max_rel, run_module, strict_fp32
+from _refmods import build_reference, have_reference, max_rel, record_parity, run_module, strict_fp32
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-5
@@ -82,8 +82,6 @@ def test_seggpt_tiny_golden_fp32_mode_auto_selected():
 def test_seggpt_vitl_run_one_image_fp32_mode_vs_reference_fp32():
     """configs[2] at full size through the UNMODIFIED seggpt_engine.run_one_image: the module in its default "auto"
     precision against the reference module in strict fp32 on the same GPU."""
-    import json
-    import os
     from oracle import ref_loader
     se = ref_loader.seggpt_engine()
     cfg = po.PainterConfig(seggpt=True)
@@ -104,14 +102,7 @@ def test_seggpt_vitl_run_one_image_fp32_mode_vs_reference_fp32():
         rep[f"P{P}_{seg}"] = {"max_abs_err_over_255": err, "max_rel": max_rel(out_o, out_f)}
         assert err <= TOL, rep
     print(rep)
-    path = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out", "r02_parity.json")
-    try:
-        allr = json.load(open(path))
-    except (OSError, ValueError):
-        allr = {}
-    allr["seggpt_vitl_run_one_image_fp32_mode"] = rep
-    os.makedirs(os.path.dirname(path), exist_ok=True)
-    json.dump(allr, open(path, "w"), indent=1, sort_keys=True)
+    record_parity("seggpt_vitl_run_one_image_fp32_mode", rep)
 
 
 @pytest.mark.skipif(not have_reference(), reason="reference tree not staged")

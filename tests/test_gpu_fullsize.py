@@ -1,10 +1,9 @@
 """GPU parity at the BENCHMARKED shapes against the UNMODIFIED reference executed on the same GPU (staged copy under
-baseline/_ref, scripts/stage_reference.py), following the SURVEY.md section 8(c) protocol:
+oracle/_ref, scripts/stage_reference.py), following the SURVEY.md section 8(c) protocol:
 
   * loss: |ours - ref| <= 1e-3 |ref| against the reference in fp32 (TF32 off) AND under torch.autocast('cuda', bf16);
   * logits / gradients: err(ours, fp32 reference) <= 1.5 x err(reference-bf16-autocast, fp32 reference), per
-    tensor (RMS-rel) and globally; the measured ratios are written to gpurun_out/r02_parity.json (committed copy:
-    profiles/r02_parity.json).
+    tensor (RMS-rel) and globally; the measured ratios go to the parity report (_refmods.record_parity).
 
 Covers BASELINE.json configs[1] (ViT-L 896x448, B=1 eval and B=8 train with the module's own CUDA DropPath draws),
 configs[2] (SegGPT ViT-L through the unmodified seggpt_engine.run_one_image, 1 and 2 prompts), configs[4] (1792x896,
@@ -12,7 +11,6 @@ N=6272: full forward + one Block forward/backward) and the unmodified engine_tra
 """
 import gc
 import json
-import os
 import types
 
 import numpy as np
@@ -23,27 +21,17 @@ from oracle import painter_oracle as po
 from oracle.synth import synth_inputs, synth_state_dict
 
 from _common import build_model
-from _refmods import (build_reference, grad_report, have_reference, max_rel, rms_rel, run_module, strict_fp32)
+from _refmods import (build_reference, grad_report, have_reference, max_rel, record_parity, rms_rel, run_module,
+                      strict_fp32)
 
 pytestmark = [pytest.mark.gpu, pytest.mark.skipif(not have_reference(), reason="reference tree not staged")]
 
 LOSS_TOL = 1e-3          # north star: loss within 1e-3 relative of the reference
 NOISE_RATIO = 1.5        # SURVEY 8(c): ours <= 1.5 x the reference's own bf16 error
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _record(name, payload):
-    d = os.path.join(ROOT, "gpurun_out")
-    os.makedirs(d, exist_ok=True)
-    path = os.path.join(d, "r02_parity.json")
-    try:
-        with open(path) as f:
-            allr = json.load(f)
-    except (OSError, ValueError):
-        allr = {}
-    allr[name] = payload
-    with open(path, "w") as f:
-        json.dump(allr, f, indent=1, sort_keys=True)
+    record_parity(name, payload)
 
 
 def _free():

@@ -1,6 +1,6 @@
 """Pins the CPU oracle (oracle/painter_oracle.py) against golden vectors produced by executing the
-unmodified reference (oracle/make_golden.py) and, where /root/reference exists, against the live
-reference.  CPU only."""
+unmodified reference (oracle/make_golden.py) and, where a copy of the reference is found (oracle/ref_loader.py),
+against the live reference.  CPU only."""
 import os
 
 import pytest
@@ -10,11 +10,7 @@ from oracle import painter_oracle as po
 from oracle import ref_loader
 from oracle.synth import fingerprint, synth_inputs, synth_state_dict
 
-from conftest import GOLDEN
-
-
-def _load(name):
-    return torch.load(os.path.join(GOLDEN, name), weights_only=False)
+from _common import load_golden as _load
 
 
 def _rel(a, b):
@@ -113,7 +109,7 @@ def test_patchify_roundtrip():
     assert torch.equal(po.unpatchify(po.patchify(x, 16), 16), x)
 
 
-@pytest.mark.skipif(not ref_loader.available(), reason="/root/reference not present")
+@pytest.mark.skipif(not ref_loader.available(), reason="reference tree not present")
 def test_live_reference_stock_constructor_is_all_global():
     """SURVEY.md §0.1: the stock factory builds 24 global-attention blocks (tuple-of-lists bug)."""
     mp = ref_loader.models_painter()
@@ -125,7 +121,7 @@ def test_live_reference_stock_constructor_is_all_global():
     assert not any(i in wbi for i in range(24))
 
 
-@pytest.mark.skipif(not ref_loader.available(), reason="reference tree not present (neither /root/reference nor baseline/_ref)")
+@pytest.mark.skipif(not ref_loader.available(), reason="reference tree not present (neither a checkout nor oracle/_ref)")
 def test_live_reference_full_size_forward_pins_the_oracle_at_the_benchmark_geometry():
     """The oracle against the UNMODIFIED reference module at the geometry the benchmark runs (ViT-L, 896x448, the stock
     factory) - not only at the toy geometry of the golden vectors: eval-mode forward, B = 1, same seeded weights and
