@@ -3,10 +3,12 @@
 // Replaces models_painter.py:73-86 + util/vitdet_utils.py:63-125 (q*scale @ k^T, add_decomposed_rel_pos, softmax,
 // @ v) and autograd's backward through them, without ever materialising the [B*heads, N, N] score tensor.
 //
-// Every kernel works on 64-row tiles with 4 warps (16 rows each) and bf16 tensor-core MMAs (mma.sync m16n8k16, fp32
-// accumulation); the probabilities P stay in registers between the two products (their accumulator fragment is the
-// A-operand fragment of the next MMA), operand tiles are staged in padded shared memory (row stride 72 bf16:
-// fragment loads are conflict-free).
+// Every kernel is one warpgroup (4 warps, warp w owns rows [16 w, 16 w + 16)) working on 64-row tiles with
+// wgmma.mma_async m64n64k16 (bf16 in, fp32 accumulation in registers).  Operand tiles live in shared memory in the
+// 128B-swizzled layout the wgmma descriptors read, filled by cp.async and double-buffered, so the loads of the next
+// tile overlap the math of this one.  A tile stored [rows][64] serves both as a K-major operand and, through the
+// descriptor's transpose bit, as an MN-major one: no transposed copies are made.  The probabilities P (and dS) stay in
+// registers between the two products: their accumulator fragment is the register A operand of the next wgmma.
 //   forward   one CTA per 64 queries of one (batch, head): S = Q K^T over 64-key tiles, online softmax in the log2
 //             domain, O += P V; writes O and the log-sum-exp.
 //   backward  dQ kernel (per 64 queries; also the bias-row gradients and the per-CTA table-gradient partials) and
@@ -15,15 +17,17 @@
 // per query, ~3 % of the attention FLOPs) are computed once per query tile on the FMA pipe and kept, log2e-scaled, in
 // shared memory; the training forward stores them for the backward kernels ([B*heads, Np, h] / [B*heads, Np, w]).
 #include "common.cuh"
+#include "wgmma.cuh"
 #include "host_common.h"
 #include "../../include/painter_b200.h"
 
 namespace pk {
 
-constexpr int AT_BM = 64;          // rows (queries or keys) per CTA and per loop tile
-constexpr int AT_THREADS = 128;
-constexpr int AT_LDS = 72;         // bf16 per staged row (64 + 8 pad)
-constexpr int AT_TILE = AT_BM * AT_LDS;   // bf16 elements of one staged 64 x 64 tile
+constexpr int AT_BM = 64;                     // rows (queries or keys) per CTA and per loop tile
+constexpr int AT_THREADS = 128;               // one warpgroup
+constexpr int AT_TILE = AT_BM * 128;          // bytes of one 64 x 64 bf16 operand tile
+constexpr int AT_TLD = 72;                    // bf16 per staged rel-pos table row (64 + 8 pad, FMA-pipe reads)
+constexpr int AT_DSLD = 65;                   // fp32 per row of the dQ kernel's dS tile (odd: conflict-free row reads)
 constexpr float AT_LOG2E = 1.4426950408889634f;
 
 struct AttnArgs {
@@ -42,96 +46,112 @@ struct AttnArgs {
   float scale_log2;           // head_dim^-0.5 * log2(e)
 };
 
-__device__ __forceinline__ void mma_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
-      "{%0, %1, %2, %3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ uint32_t lds32(const __nv_bfloat16* s, int row, int col) {
-  return *reinterpret_cast<const uint32_t*>(s + row * AT_LDS + col);
-}
 __device__ __forceinline__ float bf16lo(uint32_t u) { return __uint_as_float(u << 16); }
 __device__ __forceinline__ float bf16hi(uint32_t u) { return __uint_as_float(u & 0xFFFF0000u); }
 
-// Stage rows [r0, r0 + 64) x columns [c0, c0 + 64) of a bf16 matrix (row stride ld elements, rows >= nrows read as
-// zero): row-major into s[row][col] and/or transposed into st[col][row].
-__device__ __forceinline__ void stage_tile(const __nv_bfloat16* g, size_t ld, int r0, int nrows, int c0,
-                                           __nv_bfloat16* s, __nv_bfloat16* st) {
+// Byte offset of 16-byte chunk `ch` of row `row` in a [rows][64] bf16 tile with 128-byte swizzle (8-row atoms of
+// 1024 bytes; the tile is 1024-byte aligned), the layout SWIZZLE_128B descriptors expect.
+__device__ __forceinline__ uint32_t sw128(int row, int ch) { return row * 128 + ((ch ^ (row & 7)) << 4); }
+__device__ __forceinline__ float sw128_elem(const uint8_t* tile, int row, int col) {
+  return __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(tile + sw128(row, col >> 3) + (col & 7) * 2));
+}
+
+// cp.async with zero fill: the destination gets `bytes` bytes from src and zeros for the rest of the copy size
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async4(uint32_t dst, const void* src, uint32_t bytes) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+// Start copying rows [r0, r0 + 64) x columns [c0, c0 + 64) of a bf16 matrix (row stride ld elements, rows >= nrows
+// read as zero) into the swizzled tile at shared address s.
+__device__ __forceinline__ void load_tile(uint32_t s, const __nv_bfloat16* g, size_t ld, int r0, int nrows, int c0) {
 #pragma unroll
   for (int it = 0; it < (AT_BM * 8) / AT_THREADS; ++it) {
     const int idx = it * AT_THREADS + threadIdx.x;
-    const int row = idx >> 3, ch = idx & 7;
-    uint4 v = make_uint4(0u, 0u, 0u, 0u);
-    if (r0 + row < nrows) v = *reinterpret_cast<const uint4*>(g + static_cast<size_t>(r0 + row) * ld + c0 + ch * 8);
-    if (s != nullptr) *reinterpret_cast<uint4*>(s + row * AT_LDS + ch * 8) = v;
-    if (st != nullptr) {
-      const __nv_bfloat16* e = reinterpret_cast<const __nv_bfloat16*>(&v);
+    const int row = idx >> 3, ch = idx & 7, r = r0 + row;
+    const __nv_bfloat16* src = g + static_cast<size_t>(min(r, nrows - 1)) * ld + c0 + ch * 8;
+    cp_async16(s + sw128(row, ch), src, r < nrows ? 16u : 0u);
+  }
+}
+// The cp.async data of the waited groups becomes visible to every thread's wgmma (async proxy).
+template <int PENDING>
+__device__ __forceinline__ void tiles_ready() {
+  cp_async_wait<PENDING>();
+  fence_proxy_async_smem();
+  __syncthreads();
+}
+
+// d[64 x 64] = A . B^T: A a [64][64] tile (rows = output rows), B a [64][64] tile (rows = output columns), both
+// K-major.  Issues the wgmmas only; the caller fences, commits and waits.
+__device__ __forceinline__ void mma_ss(float (&d)[32], uint32_t sa, uint32_t sb) {
+  const uint64_t da = make_wgmma_desc(sa, 16, 1024), db = make_wgmma_desc(sb, 16, 1024);
 #pragma unroll
-      for (int k = 0; k < 8; ++k) st[(ch * 8 + k) * AT_LDS + row] = e[k];
+  for (int k = 0; k < 4; ++k)
+    wgmma_m64n64k16<0, 0>(d, wgmma_desc_add(da, k * 32), wgmma_desc_add(db, k * 32), k > 0 ? 1u : 0u);
+}
+// d[64 x 64] += P . B: P as packed register fragments (pack_frag), B a [64][64] tile (rows = the reduction index)
+// read MN-major.
+__device__ __forceinline__ void mma_rs(float (&d)[32], const uint32_t (&p)[4][4], uint32_t sb) {
+  const uint64_t db = make_wgmma_desc(sb, AT_TILE, 1024);
+#pragma unroll
+  for (int k = 0; k < 4; ++k) wgmma_m64n64k16_rs<1>(d, p[k], wgmma_desc_add(db, k * 2048), 1u);
+}
+// accumulator fragment -> bf16 A fragments of the next product (wgmma_m64n64k16_rs)
+__device__ __forceinline__ void pack_frag(const float (&s)[32], uint32_t (&p)[4][4]) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      p[k][j] = pack_bf16x2(s[8 * k + 2 * j], s[8 * k + 2 * j + 1]);
+      asm volatile("" : "+r"(p[k][j])::"memory");   // written before the wgmma.fence
     }
   }
 }
+__device__ __forceinline__ void zero32(float (&d)[32]) {
+#pragma unroll
+  for (int i = 0; i < 32; ++i) d[i] = 0.f;
+}
 
-// A-operand fragments of rows [16 warp, 16 warp + 16) x 64 of a staged row-major tile
-__device__ __forceinline__ void load_afrag(const __nv_bfloat16* s, uint32_t (&a)[4][4]) {
-  const int lane = threadIdx.x & 31, r = (threadIdx.x >> 5) * 16 + (lane >> 2), c = 2 * (lane & 3);
-#pragma unroll
-  for (int ks = 0; ks < 4; ++ks) {
-    a[ks][0] = lds32(s, r, ks * 16 + c);
-    a[ks][1] = lds32(s, r + 8, ks * 16 + c);
-    a[ks][2] = lds32(s, r, ks * 16 + c + 8);
-    a[ks][3] = lds32(s, r + 8, ks * 16 + c + 8);
-  }
-}
-// acc[16 x 64] += A[16 x 64] . B^T, B = 64 rows of a staged row-major tile (rows = output columns)
-__device__ __forceinline__ void mma_rows(float (&acc)[8][4], const uint32_t (&a)[4][4], const __nv_bfloat16* sb) {
-  const int lane = threadIdx.x & 31, g = lane >> 2, c = 2 * (lane & 3);
-#pragma unroll
-  for (int ks = 0; ks < 4; ++ks)
-#pragma unroll
-    for (int nt = 0; nt < 8; ++nt)
-      mma_16816(acc[nt], a[ks], lds32(sb, nt * 8 + g, ks * 16 + c), lds32(sb, nt * 8 + g, ks * 16 + c + 8));
-}
-// acc[16 x 64] += P[16 x 64] . B, P given as accumulator fragments (bf16-rounded here), B^T staged row-major
-__device__ __forceinline__ void mma_p(float (&acc)[8][4], const float (&p)[8][4], const __nv_bfloat16* sbt) {
-  const int lane = threadIdx.x & 31, g = lane >> 2, c = 2 * (lane & 3);
-#pragma unroll
-  for (int kk = 0; kk < 4; ++kk) {
-    const uint32_t a[4] = {pack_bf16x2(p[2 * kk][0], p[2 * kk][1]), pack_bf16x2(p[2 * kk][2], p[2 * kk][3]),
-                           pack_bf16x2(p[2 * kk + 1][0], p[2 * kk + 1][1]),
-                           pack_bf16x2(p[2 * kk + 1][2], p[2 * kk + 1][3])};
-#pragma unroll
-    for (int dt = 0; dt < 8; ++dt)
-      mma_16816(acc[dt], a, lds32(sbt, dt * 8 + g, kk * 16 + c), lds32(sbt, dt * 8 + g, kk * 16 + c + 8));
+// Stage both bf16 tables (row stride AT_TLD) into sT.
+__device__ __forceinline__ void stage_tables(const AttnArgs& a, __nv_bfloat16* sT) {
+  const int Lh = 2 * a.h - 1, Lw = 2 * a.w - 1;
+  for (int idx = threadIdx.x; idx < (Lh + Lw) * 8; idx += AT_THREADS) {
+    const int row = idx >> 3, ch = idx & 7;
+    const __nv_bfloat16* src = row < Lh ? a.th + static_cast<size_t>(row) * 64 : a.tw + static_cast<size_t>(row - Lh) * 64;
+    *reinterpret_cast<uint4*>(sT + row * AT_TLD + ch * 8) = *reinterpret_cast<const uint4*>(src + ch * 8);
   }
 }
 
 // Bias rows of the 64 queries [q0, q0 + 64) of one (batch, head), log2e-scaled, into relh_s [64][h] / relw_s [64][w]
-// (and to global when relh_g / relw_g are given).  sQ: the staged query tile; sT: scratch for both bf16 tables.
-__device__ void compute_bias_rows(const AttnArgs& a, const __nv_bfloat16* sQ, __nv_bfloat16* sT, int q0,
+// (and to global when relh_g / relw_g are given).  sQ: the swizzled query tile; sT: scratch for both bf16 tables.
+__device__ void compute_bias_rows(const AttnArgs& a, const uint8_t* sQ, __nv_bfloat16* sT, int q0,
                                   float* relh_s, float* relw_s, float* relh_g, float* relw_g) {
-  const int h = a.h, w = a.w, Lh = 2 * h - 1, Lw = 2 * w - 1;
-  for (int idx = threadIdx.x; idx < (Lh + Lw) * 8; idx += AT_THREADS) {
-    const int row = idx >> 3, ch = idx & 7;
-    const __nv_bfloat16* src = row < Lh ? a.th + static_cast<size_t>(row) * 64 : a.tw + static_cast<size_t>(row - Lh) * 64;
-    *reinterpret_cast<uint4*>(sT + row * AT_LDS + ch * 8) = *reinterpret_cast<const uint4*>(src + ch * 8);
-  }
+  const int h = a.h, w = a.w, Lh = 2 * h - 1;
+  stage_tables(a, sT);
   __syncthreads();
   for (int idx = threadIdx.x; idx < AT_BM * (h + w); idx += AT_THREADS) {
     const int q = idx / (h + w), k = idx - q * (h + w);
     const int t = min(q0 + q, a.N - 1);
     const int iq = t / w, jq = t - iq * w;
     const int trow = k < h ? iq - k + h - 1 : Lh + jq - (k - h) + w - 1;
-    const uint32_t* qa = reinterpret_cast<const uint32_t*>(sQ + q * AT_LDS);
-    const uint32_t* ta = reinterpret_cast<const uint32_t*>(sT + trow * AT_LDS);
+    const uint4* qa = reinterpret_cast<const uint4*>(sQ + q * 128);
+    const uint32_t* ta = reinterpret_cast<const uint32_t*>(sT + trow * AT_TLD);
     float s0 = 0.f, s1 = 0.f;
-#pragma unroll 8
-    for (int c = 0; c < 32; ++c) {
-      const uint32_t x = qa[c], y = ta[c];
-      s0 = fmaf(bf16lo(x), bf16lo(y), s0);
-      s1 = fmaf(bf16hi(x), bf16hi(y), s1);
+#pragma unroll
+    for (int ch = 0; ch < 8; ++ch) {
+      const uint4 x4 = qa[ch ^ (q & 7)];
+      const uint32_t x[4] = {x4.x, x4.y, x4.z, x4.w};
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const uint32_t y = ta[ch * 4 + e];
+        s0 = fmaf(bf16lo(x[e]), bf16lo(y), s0);
+        s1 = fmaf(bf16hi(x[e]), bf16hi(y), s1);
+      }
     }
     const float v = (s0 + s1) * AT_LOG2E;
     if (k < h) {
@@ -144,18 +164,36 @@ __device__ void compute_bias_rows(const AttnArgs& a, const __nv_bfloat16* sQ, __
   }
 }
 
+// Shared-memory carve-ups (bytes past the 1024-byte aligned base; the launch adds 1024 bytes of alignment slack).
+__host__ __device__ inline size_t table_bytes(int h, int w) { return static_cast<size_t>(2 * h - 1 + 2 * w - 1) * AT_TLD * 2; }
+// forward / dQ: 2-stage K | V ring, which also holds the staged tables when no tile is in flight
+__host__ __device__ inline size_t kv_ring_bytes(int h, int w) {
+  const size_t t = table_bytes(h, w);
+  return t > 4 * AT_TILE ? t : 4 * AT_TILE;
+}
+// dK/dV: one stage = Q | dO | relh rows [64][h] | relw rows [64][w] | lse [64] | delta [64]
+__host__ __device__ inline size_t dkv_stage_bytes(int h, int w) {
+  return (2 * AT_TILE + static_cast<size_t>(AT_BM) * (h + w) * 4 + 2 * AT_BM * 4 + 1023) / 1024 * 1024;
+}
+
+__device__ __forceinline__ uint8_t* aligned_smem(uint8_t* raw, uint32_t& base) {
+  const uint32_t r = smem_u32(raw);
+  base = (r + 1023u) & ~1023u;
+  return raw + (base - r);
+}
+
 // ------------------------------------------------------------------------------------------------------------------
 // forward.  grid (query tiles, heads, B)
-// smem: sQ | sK | sVt | tables (2h-1 + 2w-1 rows) | relh_s [64][h] | relw_s [64][w]
+// smem: sQ | K/V ring (tables before the loop) | relh_s [64][h] | relw_s [64][w]
 __global__ void __launch_bounds__(AT_THREADS)
 attn_fwd_kernel(const AttnArgs a) {
-  extern __shared__ __align__(16) uint8_t smem_raw[];
-  __nv_bfloat16* sQ = reinterpret_cast<__nv_bfloat16*>(smem_raw);
-  __nv_bfloat16* sK = sQ + AT_TILE;
-  __nv_bfloat16* sVt = sK + AT_TILE;
-  __nv_bfloat16* sT = sVt + AT_TILE;
+  extern __shared__ uint8_t smem_raw[];
+  uint32_t sQ;
+  uint8_t* sm = aligned_smem(smem_raw, sQ);
+  const uint32_t ring = sQ + AT_TILE;
   const int h = a.h, w = a.w, N = a.N, C = a.heads * 64;
-  float* relh_s = reinterpret_cast<float*>(sT + (2 * h - 1 + 2 * w - 1) * AT_LDS);
+  __nv_bfloat16* sT = reinterpret_cast<__nv_bfloat16*>(sm + AT_TILE);
+  float* relh_s = reinterpret_cast<float*>(sm + AT_TILE + kv_ring_bytes(h, w));
   float* relw_s = relh_s + AT_BM * h;
   const int q0 = blockIdx.x * AT_BM, head = blockIdx.y, b = blockIdx.z;
   const size_t bh = static_cast<size_t>(b) * a.heads + head;
@@ -163,30 +201,44 @@ attn_fwd_kernel(const AttnArgs a) {
   pdl_launch_dependents();
   pdl_wait();
 
-  stage_tile(base, 3 * C, q0, N, head * 64, sQ, nullptr);
+  load_tile(sQ, base, 3 * C, q0, N, head * 64);
+  cp_async_commit();
+  cp_async_wait<0>();
   __syncthreads();
-  compute_bias_rows(a, sQ, sT, q0, relh_s, relw_s, a.relh ? a.relh + bh * a.Np * h : nullptr,
+  compute_bias_rows(a, sm, sT, q0, relh_s, relw_s, a.relh ? a.relh + bh * a.Np * h : nullptr,
                     a.relw ? a.relw + bh * a.Np * w : nullptr);
-  uint32_t qa[4][4];
-  load_afrag(sQ, qa);
+  __syncthreads();   // the tables are dead: the ring takes their place
+
+  const int ntiles = (N + AT_BM - 1) / AT_BM;
+  auto issue = [&](int t) {
+    if (t < ntiles) {
+      const uint32_t st = ring + (t & 1) * 2 * AT_TILE;
+      load_tile(st, base, 3 * C, t * AT_BM, N, C + head * 64);
+      load_tile(st + AT_TILE, base, 3 * C, t * AT_BM, N, 2 * C + head * 64);
+    }
+    cp_async_commit();
+  };
+  issue(0);
 
   const int lane = threadIdx.x & 31, g = lane >> 2, c2 = 2 * (lane & 3);
   const int rl0 = (threadIdx.x >> 5) * 16 + g;     // local query rows rl0, rl0 + 8
   const float sc = a.scale_log2;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
-  float o[8][4];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
+  float o[32], s[32];
+  zero32(o);
+  zero32(s);
 
-  for (int k0 = 0; k0 < N; k0 += AT_BM) {
-    __syncthreads();
-    stage_tile(base, 3 * C, k0, N, C + head * 64, sK, nullptr);
-    stage_tile(base, 3 * C, k0, N, 2 * C + head * 64, nullptr, sVt);
-    __syncthreads();
-    float s[8][4];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f;
-    mma_rows(s, qa, sK);
+  for (int t = 0; t < ntiles; ++t) {
+    issue(t + 1);
+    tiles_ready<1>();
+    const uint32_t sK = ring + (t & 1) * 2 * AT_TILE, sV = sK + AT_TILE;
+    const int k0 = t * AT_BM;
+    wgmma_fence_operands(s);
+    wgmma_fence();
+    mma_ss(s, sQ, sK);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operands(s);
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt)
@@ -196,9 +248,9 @@ attn_fwd_kernel(const AttnArgs a) {
         float v = -INFINITY;
         if (key < N) {
           const int kr = key / w, kc = key - kr * w;
-          v = fmaf(s[nt][e], sc, relh_s[r * h + kr] + relw_s[r * w + kc]);
+          v = fmaf(s[4 * nt + e], sc, relh_s[r * h + kr] + relw_s[r * w + kc]);
         }
-        s[nt][e] = v;
+        s[4 * nt + e] = v;
         mx[e >> 1] = fmaxf(mx[e >> 1], v);
       }
     float alpha[2];
@@ -212,15 +264,21 @@ attn_fwd_kernel(const AttnArgs a) {
       l[i] *= alpha[i];
     }
 #pragma unroll
-    for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float p = fast_exp2(s[nt][e] - m[e >> 1]);
-        s[nt][e] = p;
-        l[e >> 1] += p;
-        o[nt][e] *= alpha[e >> 1];
-      }
-    mma_p(o, s, sVt);
+    for (int i = 0; i < 32; ++i) {
+      const float p = fast_exp2(s[i] - m[(i >> 1) & 1]);
+      s[i] = p;
+      l[(i >> 1) & 1] += p;
+      o[i] *= alpha[(i >> 1) & 1];
+    }
+    uint32_t pa[4][4];
+    pack_frag(s, pa);
+    wgmma_fence_operands(o);
+    wgmma_fence();
+    mma_rs(o, pa, sV);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operands(o);
+    __syncthreads();   // stage t & 1 is free for tile t + 2
   }
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
@@ -235,62 +293,73 @@ attn_fwd_kernel(const AttnArgs a) {
     __nv_bfloat16* orow = a.out + (static_cast<size_t>(b) * N + t) * C + head * 64;
 #pragma unroll
     for (int dt = 0; dt < 8; ++dt)
-      *reinterpret_cast<uint32_t*>(orow + dt * 8 + c2) = pack_bf16x2(o[dt][2 * i] * inv, o[dt][2 * i + 1] * inv);
+      *reinterpret_cast<uint32_t*>(orow + dt * 8 + c2) =
+          pack_bf16x2(o[4 * dt + 2 * i] * inv, o[4 * dt + 2 * i + 1] * inv);
     if (a.lse && (lane & 3) == 0) a.lse[bh * N + t] = m[i] + log2f(l[i]);
   }
 }
 
 // bias rows only (pk_attn_bwd without rows kept by the forward).  grid (query tiles, heads, B)
+// smem: sQ | tables | relh_s | relw_s
 __global__ void __launch_bounds__(AT_THREADS)
 attn_bias_rows_kernel(const AttnArgs a) {
-  extern __shared__ __align__(16) uint8_t smem_raw[];
-  __nv_bfloat16* sQ = reinterpret_cast<__nv_bfloat16*>(smem_raw);
-  __nv_bfloat16* sT = sQ + AT_TILE;
+  extern __shared__ uint8_t smem_raw[];
+  uint32_t sQ;
+  uint8_t* sm = aligned_smem(smem_raw, sQ);
   const int h = a.h, w = a.w, N = a.N, C = a.heads * 64;
-  float* relh_s = reinterpret_cast<float*>(sT + (2 * h - 1 + 2 * w - 1) * AT_LDS);
+  __nv_bfloat16* sT = reinterpret_cast<__nv_bfloat16*>(sm + AT_TILE);
+  float* relh_s = reinterpret_cast<float*>(sm + AT_TILE + table_bytes(h, w));
   float* relw_s = relh_s + AT_BM * h;
   const int q0 = blockIdx.x * AT_BM, head = blockIdx.y, b = blockIdx.z;
   const size_t bh = static_cast<size_t>(b) * a.heads + head;
   pdl_launch_dependents();
   pdl_wait();
-  stage_tile(a.qkv + static_cast<size_t>(b) * N * 3 * C, 3 * C, q0, N, head * 64, sQ, nullptr);
+  load_tile(sQ, a.qkv + static_cast<size_t>(b) * N * 3 * C, 3 * C, q0, N, head * 64);
+  cp_async_commit();
+  cp_async_wait<0>();
   __syncthreads();
-  compute_bias_rows(a, sQ, sT, q0, relh_s, relw_s, a.relh + bh * a.Np * h, a.relw + bh * a.Np * w);
+  compute_bias_rows(a, sm, sT, q0, relh_s, relw_s, a.relh + bh * a.Np * h, a.relw + bh * a.Np * w);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
 // backward, dQ side.  grid (query tiles, heads, B)
 //   dS = P * (dP - delta),  dQ = scale dS K + dRelh . T_h(gathered) + dRelw . T_w(gathered)
-//   dRelh[q, i] = sum of dS over the keys of image row i, dRelw[q, j] over image column j (shared-memory atomics)
+//   dRelh[q, i] = sum of dS over the keys of image row i, dRelw[q, j] over image column j (each key tile's dS goes
+//   through shared memory and is summed by the owner threads of the row)
 //   table-gradient partials: ws[cta][c][r] = sum_q dRel[q, .] q[c] over the (q, bias column) pairs hitting table row r
-// smem: sQ | sdO | sK | sKt | sV | tables | relh_s | relw_s | drelh_s | drelw_s
+// smem: sQ | sdO | K/V ring (tables after the loop) | relh_s | relw_s | drelh_s | drelw_s | ds_s [64][AT_DSLD]
 __global__ void __launch_bounds__(AT_THREADS)
 attn_bwd_dq_kernel(const AttnArgs a) {
-  extern __shared__ __align__(16) uint8_t smem_raw[];
-  __nv_bfloat16* sQ = reinterpret_cast<__nv_bfloat16*>(smem_raw);
-  __nv_bfloat16* sdO = sQ + AT_TILE;
-  __nv_bfloat16* sK = sdO + AT_TILE;
-  __nv_bfloat16* sKt = sK + AT_TILE;
-  __nv_bfloat16* sV = sKt + AT_TILE;
-  __nv_bfloat16* sT = sV + AT_TILE;
+  extern __shared__ uint8_t smem_raw[];
+  uint32_t sQ;
+  uint8_t* sm = aligned_smem(smem_raw, sQ);
+  const uint32_t sdO = sQ + AT_TILE, ring = sdO + AT_TILE;
   const int h = a.h, w = a.w, N = a.N, C = a.heads * 64, Lh = 2 * h - 1, Lw = 2 * w - 1;
-  float* relh_s = reinterpret_cast<float*>(sT + (Lh + Lw) * AT_LDS);
+  __nv_bfloat16* sT = reinterpret_cast<__nv_bfloat16*>(sm + 2 * AT_TILE);
+  float* relh_s = reinterpret_cast<float*>(sm + 2 * AT_TILE + kv_ring_bytes(h, w));
   float* relw_s = relh_s + AT_BM * h;
   float* drelh_s = relw_s + AT_BM * w;
   float* drelw_s = drelh_s + AT_BM * h;
+  float* ds_s = drelw_s + AT_BM * w;
   const int q0 = blockIdx.x * AT_BM, head = blockIdx.y, b = blockIdx.z;
   const size_t bh = static_cast<size_t>(b) * a.heads + head;
   const __nv_bfloat16* base = a.qkv + static_cast<size_t>(b) * N * 3 * C;
   pdl_launch_dependents();
   pdl_wait();
 
-  stage_tile(base, 3 * C, q0, N, head * 64, sQ, nullptr);
-  stage_tile(a.dO + static_cast<size_t>(b) * N * C, C, q0, N, head * 64, sdO, nullptr);
-  for (int idx = threadIdx.x; idx < (Lh + Lw) * 8; idx += AT_THREADS) {
-    const int row = idx >> 3, ch = idx & 7;
-    const __nv_bfloat16* src = row < Lh ? a.th + static_cast<size_t>(row) * 64 : a.tw + static_cast<size_t>(row - Lh) * 64;
-    *reinterpret_cast<uint4*>(sT + row * AT_LDS + ch * 8) = *reinterpret_cast<const uint4*>(src + ch * 8);
-  }
+  load_tile(sQ, base, 3 * C, q0, N, head * 64);
+  load_tile(sdO, a.dO + static_cast<size_t>(b) * N * C, C, q0, N, head * 64);
+  cp_async_commit();
+  const int ntiles = (N + AT_BM - 1) / AT_BM;
+  auto issue = [&](int t) {
+    if (t < ntiles) {
+      const uint32_t st = ring + (t & 1) * 2 * AT_TILE;
+      load_tile(st, base, 3 * C, t * AT_BM, N, C + head * 64);
+      load_tile(st + AT_TILE, base, 3 * C, t * AT_BM, N, 2 * C + head * 64);
+    }
+    cp_async_commit();
+  };
+  issue(0);
   {
     const float* gh = a.relh + (bh * a.Np + q0) * h;
     const float* gw = a.relw + (bh * a.Np + q0) * w;
@@ -303,13 +372,10 @@ attn_bwd_dq_kernel(const AttnArgs a) {
       drelw_s[i] = 0.f;
     }
   }
-  __syncthreads();
-  uint32_t qa[4][4], da[4][4];
-  load_afrag(sQ, qa);
-  load_afrag(sdO, da);
 
   const int lane = threadIdx.x & 31, g = lane >> 2, c2 = 2 * (lane & 3);
   const int rl0 = (threadIdx.x >> 5) * 16 + g;
+  const int own_r = threadIdx.x >> 1, part = threadIdx.x & 1;   // a row of this thread's own warp
   const float sc = a.scale_log2;
   float lse[2], dlt[2];
 #pragma unroll
@@ -318,20 +384,25 @@ attn_bwd_dq_kernel(const AttnArgs a) {
     lse[i] = a.lse[bh * N + t];
     dlt[i] = a.delta[bh * N + t];
   }
-  float dq[8][4];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f;
+  float dq[32], s[32], dp[32];
+  zero32(dq);
+  zero32(s);
+  zero32(dp);
 
-  for (int k0 = 0; k0 < N; k0 += AT_BM) {
-    __syncthreads();
-    stage_tile(base, 3 * C, k0, N, C + head * 64, sK, sKt);
-    stage_tile(base, 3 * C, k0, N, 2 * C + head * 64, sV, nullptr);
-    __syncthreads();
-    float s[8][4], dp[8][4];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = dp[i][0] = dp[i][1] = dp[i][2] = dp[i][3] = 0.f;
-    mma_rows(s, qa, sK);
-    mma_rows(dp, da, sV);
+  for (int t = 0; t < ntiles; ++t) {
+    issue(t + 1);
+    tiles_ready<1>();
+    const uint32_t sK = ring + (t & 1) * 2 * AT_TILE, sV = sK + AT_TILE;
+    const int k0 = t * AT_BM;
+    wgmma_fence_operands(s);
+    wgmma_fence_operands(dp);
+    wgmma_fence();
+    mma_ss(s, sQ, sK);
+    mma_ss(dp, sdO, sV);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operands(s);
+    wgmma_fence_operands(dp);
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt)
 #pragma unroll
@@ -340,16 +411,49 @@ attn_bwd_dq_kernel(const AttnArgs a) {
         float ds = 0.f;
         if (key < N) {
           const int kr = key / w, kc = key - kr * w;
-          const float p = fast_exp2(fmaf(s[nt][e], sc, relh_s[r * h + kr] + relw_s[r * w + kc]) - lse[e >> 1]);
-          ds = p * (dp[nt][e] - dlt[e >> 1]);
-          atomicAdd(drelh_s + r * h + kr, ds);
-          atomicAdd(drelw_s + r * w + kc, ds);
+          const float p = fast_exp2(fmaf(s[4 * nt + e], sc, relh_s[r * h + kr] + relw_s[r * w + kc]) - lse[e >> 1]);
+          ds = p * (dp[4 * nt + e] - dlt[e >> 1]);
         }
-        s[nt][e] = ds;
+        s[4 * nt + e] = ds;
+        ds_s[r * AT_DSLD + nt * 8 + c2 + (e & 1)] = ds;
       }
-    mma_p(dq, s, sKt);
+    uint32_t da[4][4];
+    pack_frag(s, da);
+    __syncwarp();   // the warp's 16 rows of dS are in ds_s
+    {
+      // bias-row gradients: thread pair (2 own_r, 2 own_r + 1) owns row own_r of the warp's rows; the even thread
+      // takes the even image columns / key-tile image rows, the odd one the odd ones.  Every (row, column) has one
+      // owner, so plain adds in a fixed order: deterministic, no atomics.
+      const float* dsr = ds_s + own_r * AT_DSLD;
+      const int xn = min(AT_BM, N - k0), k0m = k0 % w, kr0 = k0 / w;
+      float* drw = drelw_s + own_r * w;
+      for (int c = part; c < w; c += 2) {
+        int x = c - k0m;
+        if (x < 0) x += w;
+        float acc = 0.f;
+        for (; x < xn; x += w) acc += dsr[x];
+        drw[c] += acc;
+      }
+      float* drh = drelh_s + own_r * h;
+      const int nslots = (k0 + xn - 1) / w - kr0 + 1;
+      for (int j = part; j < nslots; j += 2) {
+        const int xa = max(0, (kr0 + j) * w - k0), xb = min(xn, (kr0 + j + 1) * w - k0);
+        float acc = 0.f;
+        for (int x = xa; x < xb; ++x) acc += dsr[x];
+        drh[kr0 + j] += acc;
+      }
+    }
+    wgmma_fence_operands(dq);
+    wgmma_fence();
+    mma_rs(dq, da, sK);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operands(dq);
+    __syncthreads();   // stage t & 1 is free for tile t + 2
   }
-  __syncthreads();   // drelh_s / drelw_s complete
+  cp_async_wait<0>();
+  stage_tables(a, sT);
+  __syncthreads();   // tables staged, drelh_s / drelw_s complete
 
   // dQ = scale dS K + gathered table rows, written into the q columns of dqkv
 #pragma unroll
@@ -359,12 +463,12 @@ attn_bwd_dq_kernel(const AttnArgs a) {
     float acc[16];
 #pragma unroll
     for (int dt = 0; dt < 8; ++dt) {
-      acc[2 * dt] = dq[dt][2 * i] * 0.125f;
-      acc[2 * dt + 1] = dq[dt][2 * i + 1] * 0.125f;
+      acc[2 * dt] = dq[4 * dt + 2 * i] * 0.125f;
+      acc[2 * dt + 1] = dq[4 * dt + 2 * i + 1] * 0.125f;
     }
     for (int k = 0; k < h; ++k) {
       const float d = drelh_s[r * h + k];
-      const __nv_bfloat16* trow = sT + (iq - k + h - 1) * AT_LDS + c2;
+      const __nv_bfloat16* trow = sT + (iq - k + h - 1) * AT_TLD + c2;
 #pragma unroll
       for (int dt = 0; dt < 8; ++dt) {
         const uint32_t u = *reinterpret_cast<const uint32_t*>(trow + dt * 8);
@@ -374,7 +478,7 @@ attn_bwd_dq_kernel(const AttnArgs a) {
     }
     for (int k = 0; k < w; ++k) {
       const float d = drelw_s[r * w + k];
-      const __nv_bfloat16* trow = sT + (Lh + jq - k + w - 1) * AT_LDS + c2;
+      const __nv_bfloat16* trow = sT + (Lh + jq - k + w - 1) * AT_TLD + c2;
 #pragma unroll
       for (int dt = 0; dt < 8; ++dt) {
         const uint32_t u = *reinterpret_cast<const uint32_t*>(trow + dt * 8);
@@ -393,21 +497,25 @@ attn_bwd_dq_kernel(const AttnArgs a) {
   // table-gradient partials of this CTA (every entry of the slice is written)
   const int rows = Lh + Lw;
   float* ws = a.dt_ws + ((bh * gridDim.x) + blockIdx.x) * static_cast<size_t>(rows) * 64;
+  // Only the queries whose bias column hits table row r contribute: per image row ir of the tile, table row r < Lh
+  // takes column i = ir + h - 1 - r of every query in that image row, and table row Lh + rw takes column
+  // j = jq + w - 1 - rw of the queries with jq in [rw - w + 1, rw]; both are contiguous query ranges.
   const int qn = min(AT_BM, N - q0);
+  const int ir0 = q0 / w, ir1 = (q0 + qn - 1) / w;
   for (int idx = threadIdx.x; idx < rows * 64; idx += AT_THREADS) {
     const int c = idx / rows, r = idx - c * rows;
     float acc = 0.f;
-    for (int q = 0; q < qn; ++q) {
-      const int t = q0 + q, iq = t / w, jq = t - iq * w;
-      float d;
+    for (int ir = ir0; ir <= ir1; ++ir) {
+      const int ta = max(q0, ir * w), tb = min(q0 + qn, (ir + 1) * w);
       if (r < Lh) {
-        const int i = iq + h - 1 - r;
-        d = (i >= 0 && i < h) ? drelh_s[q * h + i] : 0.f;
+        const int i = ir + h - 1 - r;
+        if (i < 0 || i >= h) continue;
+        for (int t = ta; t < tb; ++t) acc = fmaf(drelh_s[(t - q0) * h + i], sw128_elem(sm, t - q0, c), acc);
       } else {
-        const int j = jq + w - 1 - (r - Lh);
-        d = (j >= 0 && j < w) ? drelw_s[q * w + j] : 0.f;
+        const int rw = r - Lh, jofs = w - 1 - rw - ir * w;   // j = t + jofs
+        for (int t = max(ta, ir * w + rw - w + 1); t < min(tb, ir * w + rw + 1); ++t)
+          acc = fmaf(drelw_s[(t - q0) * w + t + jofs], sw128_elem(sm, t - q0, c), acc);
       }
-      acc = fmaf(d, __bfloat162float(sQ[q * AT_LDS + c]), acc);
     }
     ws[idx] = acc;
   }
@@ -416,21 +524,17 @@ attn_bwd_dq_kernel(const AttnArgs a) {
 // ------------------------------------------------------------------------------------------------------------------
 // backward, dK / dV side.  grid (key tiles, heads, B); each warp owns 16 keys, the loop runs over the query tiles
 //   P^T = exp2(scale K Q^T + bias - lse),  dV += P^T dO,  dS^T = P^T * (V dO^T - delta),  dK += scale dS^T Q
-// smem: sK | sV | sQ | sQt | sdO | sdOt | relh_s [64][h] | relw_s [64][w] | lse_s [64] | dlt_s [64]
+// smem: sK | sV | STAGES x (sQ | sdO | relh rows [64][h] | relw rows [64][w] | lse [64] | delta [64])
+// STAGES = 2 overlaps the next query tile's loads with this one's math; 1 keeps two CTAs per SM on large grids.
+template <int STAGES>
 __global__ void __launch_bounds__(AT_THREADS)
 attn_bwd_dkv_kernel(const AttnArgs a) {
-  extern __shared__ __align__(16) uint8_t smem_raw[];
-  __nv_bfloat16* sK = reinterpret_cast<__nv_bfloat16*>(smem_raw);
-  __nv_bfloat16* sV = sK + AT_TILE;
-  __nv_bfloat16* sQ = sV + AT_TILE;
-  __nv_bfloat16* sQt = sQ + AT_TILE;
-  __nv_bfloat16* sdO = sQt + AT_TILE;
-  __nv_bfloat16* sdOt = sdO + AT_TILE;
+  extern __shared__ uint8_t smem_raw[];
+  uint32_t sK;
+  uint8_t* sm = aligned_smem(smem_raw, sK);
+  const uint32_t sV = sK + AT_TILE, ring = sV + AT_TILE;
   const int h = a.h, w = a.w, N = a.N, C = a.heads * 64;
-  float* relh_s = reinterpret_cast<float*>(sdOt + AT_TILE);
-  float* relw_s = relh_s + AT_BM * h;
-  float* lse_s = relw_s + AT_BM * w;
-  float* dlt_s = lse_s + AT_BM;
+  const uint32_t stage_bytes = static_cast<uint32_t>(dkv_stage_bytes(h, w));
   const int k0 = blockIdx.x * AT_BM, head = blockIdx.y, b = blockIdx.z;
   const size_t bh = static_cast<size_t>(b) * a.heads + head;
   const __nv_bfloat16* base = a.qkv + static_cast<size_t>(b) * N * 3 * C;
@@ -438,12 +542,30 @@ attn_bwd_dkv_kernel(const AttnArgs a) {
   pdl_launch_dependents();
   pdl_wait();
 
-  stage_tile(base, 3 * C, k0, N, C + head * 64, sK, nullptr);
-  stage_tile(base, 3 * C, k0, N, 2 * C + head * 64, sV, nullptr);
-  __syncthreads();
-  uint32_t ka[4][4], va[4][4];
-  load_afrag(sK, ka);
-  load_afrag(sV, va);
+  load_tile(sK, base, 3 * C, k0, N, C + head * 64);
+  load_tile(sV, base, 3 * C, k0, N, 2 * C + head * 64);
+  cp_async_commit();
+  const int ntiles = (N + AT_BM - 1) / AT_BM;
+  auto issue = [&](int t) {
+    if (t < ntiles) {
+      const int q0 = t * AT_BM;
+      const uint32_t st = ring + (t % STAGES) * stage_bytes;
+      load_tile(st, base, 3 * C, q0, N, head * 64);
+      load_tile(st + AT_TILE, dObase, C, q0, N, head * 64);
+      const uint32_t srh = st + 2 * AT_TILE, srw = srh + AT_BM * h * 4, sl = srw + AT_BM * w * 4;
+      const float* gh = a.relh + (bh * a.Np + q0) * h;   // 64 rows: inside the Np-row buffer
+      const float* gw = a.relw + (bh * a.Np + q0) * w;
+      for (int i = threadIdx.x; i < AT_BM * h / 4; i += AT_THREADS) cp_async16(srh + 16 * i, gh + 4 * i, 16u);
+      for (int i = threadIdx.x; i < AT_BM * w / 4; i += AT_THREADS) cp_async16(srw + 16 * i, gw + 4 * i, 16u);
+      const int q = threadIdx.x & (AT_BM - 1), qc = min(q0 + q, N - 1);
+      const uint32_t bytes = q0 + q < N ? 4u : 0u;
+      if (threadIdx.x < AT_BM) cp_async4(sl + 4 * q, a.lse + bh * N + qc, bytes);
+      else cp_async4(sl + AT_BM * 4 + 4 * q, a.delta + bh * N + qc, bytes);
+    }
+    cp_async_commit();
+  };
+#pragma unroll
+  for (int t = 0; t < STAGES - 1; ++t) issue(t);
 
   const int lane = threadIdx.x & 31, g = lane >> 2, c2 = 2 * (lane & 3);
   const int kl0 = (threadIdx.x >> 5) * 16 + g;     // local key rows kl0, kl0 + 8
@@ -457,45 +579,54 @@ attn_bwd_dkv_kernel(const AttnArgs a) {
     kc[i] = min(key, N - 1) - kr[i] * w;
   }
   const float sc = a.scale_log2;
-  float dk[8][4], dv[8][4];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) dk[i][0] = dk[i][1] = dk[i][2] = dk[i][3] = dv[i][0] = dv[i][1] = dv[i][2] = dv[i][3] = 0.f;
+  float dk[32], dv[32], s[32], dp[32];
+  zero32(dk);
+  zero32(dv);
+  zero32(s);
+  zero32(dp);
 
-  for (int q0 = 0; q0 < N; q0 += AT_BM) {
-    __syncthreads();
-    stage_tile(base, 3 * C, q0, N, head * 64, sQ, sQt);
-    stage_tile(dObase, C, q0, N, head * 64, sdO, sdOt);
-    {
-      const int qn = min(AT_BM, N - q0);
-      const float* gh = a.relh + (bh * a.Np + q0) * h;
-      const float* gw = a.relw + (bh * a.Np + q0) * w;
-      for (int i = threadIdx.x; i < qn * h; i += AT_THREADS) relh_s[i] = gh[i];
-      for (int i = threadIdx.x; i < qn * w; i += AT_THREADS) relw_s[i] = gw[i];
-      for (int i = threadIdx.x; i < AT_BM; i += AT_THREADS) {
-        const bool v = i < qn;
-        lse_s[i] = v ? a.lse[bh * N + q0 + i] : INFINITY;   // queries past N: p = exp2(-inf) = 0
-        dlt_s[i] = v ? a.delta[bh * N + q0 + i] : 0.f;
-      }
-    }
-    __syncthreads();
-    float s[8][4], dp[8][4];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = dp[i][0] = dp[i][1] = dp[i][2] = dp[i][3] = 0.f;
-    mma_rows(s, ka, sQ);
-    mma_rows(dp, va, sdO);
+  for (int t = 0; t < ntiles; ++t) {
+    issue(t + STAGES - 1);
+    tiles_ready<STAGES - 1>();
+    const int q0 = t * AT_BM;
+    const uint32_t sQ = ring + (t % STAGES) * stage_bytes, sdO = sQ + AT_TILE;
+    const float* relh_s = reinterpret_cast<const float*>(sm + (sQ - sK) + 2 * AT_TILE);
+    const float* relw_s = relh_s + AT_BM * h;
+    const float* lse_s = relw_s + AT_BM * w;
+    const float* dlt_s = lse_s + AT_BM;
+    wgmma_fence_operands(s);
+    wgmma_fence_operands(dp);
+    wgmma_fence();
+    mma_ss(s, sK, sQ);
+    mma_ss(dp, sV, sdO);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operands(s);
+    wgmma_fence_operands(dp);
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt)
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         const int q = nt * 8 + c2 + (e & 1), i = e >> 1;
         float p = 0.f;
-        if (kvalid[i] && lse_s[q] != INFINITY)
-          p = fast_exp2(fmaf(s[nt][e], sc, relh_s[q * h + kr[i]] + relw_s[q * w + kc[i]]) - lse_s[q]);
-        s[nt][e] = p;
-        dp[nt][e] = p * (dp[nt][e] - dlt_s[q]);
+        if (kvalid[i] && q0 + q < N)
+          p = fast_exp2(fmaf(s[4 * nt + e], sc, relh_s[q * h + kr[i]] + relw_s[q * w + kc[i]]) - lse_s[q]);
+        s[4 * nt + e] = p;
+        dp[4 * nt + e] = p * (dp[4 * nt + e] - dlt_s[q]);
       }
-    mma_p(dv, s, sdOt);
-    mma_p(dk, dp, sQt);
+    uint32_t pa[4][4], da[4][4];
+    pack_frag(s, pa);
+    pack_frag(dp, da);
+    wgmma_fence_operands(dv);
+    wgmma_fence_operands(dk);
+    wgmma_fence();
+    mma_rs(dv, pa, sdO);
+    mma_rs(dk, da, sQ);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operands(dv);
+    wgmma_fence_operands(dk);
+    __syncthreads();   // this stage is free for tile t + STAGES
   }
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
@@ -505,8 +636,8 @@ attn_bwd_dkv_kernel(const AttnArgs a) {
 #pragma unroll
     for (int dt = 0; dt < 8; ++dt) {
       *reinterpret_cast<uint32_t*>(row + C + dt * 8 + c2) =
-          pack_bf16x2(dk[dt][2 * i] * 0.125f, dk[dt][2 * i + 1] * 0.125f);
-      *reinterpret_cast<uint32_t*>(row + 2 * C + dt * 8 + c2) = pack_bf16x2(dv[dt][2 * i], dv[dt][2 * i + 1]);
+          pack_bf16x2(dk[4 * dt + 2 * i] * 0.125f, dk[4 * dt + 2 * i + 1] * 0.125f);
+      *reinterpret_cast<uint32_t*>(row + 2 * C + dt * 8 + c2) = pack_bf16x2(dv[4 * dt + 2 * i], dv[4 * dt + 2 * i + 1]);
     }
   }
 }
@@ -581,8 +712,6 @@ attn_dt_reduce_kernel(const float* __restrict__ ws, int nctas, int rows, int row
   }
 }
 
-static size_t table_bytes(int h, int w) { return static_cast<size_t>(2 * h - 1 + 2 * w - 1) * AT_LDS * 2; }
-
 static int attn_check(const void* qkv, const void* th, const void* tw, int B, int heads, int h, int w, int th_pad,
                       int tw_pad, const char* who) {
   PK_CHECK(qkv && th && tw, "%s: null pointer", who);
@@ -628,7 +757,7 @@ static int attn_fwd_impl(const void* qkv, const void* th, const void* tw, void* 
   a.lse = lse;
   a.relh = relh_out;
   a.relw = relw_out;
-  const size_t smem = 3 * AT_TILE * 2 + table_bytes(h, w) + static_cast<size_t>(AT_BM) * (h + w) * 4;
+  const size_t smem = 1024 + AT_TILE + kv_ring_bytes(h, w) + static_cast<size_t>(AT_BM) * (h + w) * 4;
   dim3 grid((a.N + AT_BM - 1) / AT_BM, heads, B);
   return launch_attn(attn_fwd_kernel, grid, smem, static_cast<cudaStream_t>(stream), a, "pk_attn_fwd");
 }
@@ -681,7 +810,7 @@ static int attn_bwd_impl(const void* qkv, const void* O, const void* dO, const f
   const dim3 grid((N + AT_BM - 1) / AT_BM, heads, B);
   const size_t rel_bytes = static_cast<size_t>(AT_BM) * (h + w) * 4;
   if (!rel_ready) {
-    if (launch_attn(attn_bias_rows_kernel, grid, AT_TILE * 2 + table_bytes(h, w) + rel_bytes, st, a,
+    if (launch_attn(attn_bias_rows_kernel, grid, 1024 + AT_TILE + table_bytes(h, w) + rel_bytes, st, a,
                     "pk_attn_bwd(bias rows)"))
       return 2;
   }
@@ -691,11 +820,18 @@ static int attn_bwd_impl(const void* qkv, const void* O, const void* dO, const f
                static_cast<const __nv_bfloat16*>(O), static_cast<const __nv_bfloat16*>(dO), delta, B, N, heads);
     PK_LAUNCH_CHECK("pk_attn_bwd(delta)");
   }
-  if (launch_attn(attn_bwd_dq_kernel, grid, 5 * AT_TILE * 2 + table_bytes(h, w) + 2 * rel_bytes, st, a,
+  if (launch_attn(attn_bwd_dq_kernel, grid,
+                  1024 + 2 * AT_TILE + kv_ring_bytes(h, w) + 2 * rel_bytes + AT_BM * AT_DSLD * 4, st, a,
                   "pk_attn_bwd(dq)"))
     return 2;
-  if (launch_attn(attn_bwd_dkv_kernel, grid, 6 * AT_TILE * 2 + rel_bytes + 2 * AT_BM * 4, st, a, "pk_attn_bwd(dkv)"))
-    return 2;
+  {
+    // two query-tile stages while two CTAs still fit on an SM (228 KB, 1 KB reserved per CTA), else one
+    const size_t smem1 = 1024 + 2 * AT_TILE + dkv_stage_bytes(h, w), smem2 = smem1 + dkv_stage_bytes(h, w);
+    const bool two = smem2 <= 113 * 1024;
+    if (launch_attn(two ? attn_bwd_dkv_kernel<2> : attn_bwd_dkv_kernel<1>, grid, two ? smem2 : smem1, st, a,
+                    "pk_attn_bwd(dkv)"))
+      return 2;
+  }
   {
     const int rows = 2 * h - 1 + 2 * w - 1;
     const int nctas = static_cast<int>(grid.x * grid.y * grid.z);

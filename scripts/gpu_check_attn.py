@@ -135,7 +135,116 @@ def _run_fwd_checks(res, qkv, th, tw, out, lse, B, heads, h, w):
         res["tflops"] = 4.0 * B * heads * N * N * 64 / ms / 1e9
 
 
+# Kernel-level timing of the training path (attn_fwd(save_rel=True) + attn_bwd(rel=...)) at the bench geometries.
+# `--bench LIB [LIB ...]` times each library in its own process (PK_LIB selects it), alternating over
+# $ATTN_BENCH_ROUNDS rounds, and compares every arm's outputs with the first arm's on the same seeded operands.
+BENCH_GEOMS = [("train_b8", 8, 16, 56, 28), ("long_b2", 2, 16, 112, 56)]
+
+
+def attn_flops(B, heads, h, w):
+    """(forward, backward) FLOPs as executed: 2 resp. 7 N x N x 64 products per (batch, head)."""
+    n2 = B * heads * (h * w) ** 2 * 64 * 2.0
+    return 2 * n2, 7 * n2
+
+
+def bench_arm(geom, iters, dump):
+    import torch
+    from painter_b200 import ops
+    name, B, heads, h, w = next(g for g in BENCH_GEOMS if g[0] == geom)
+    N, C = h * w, heads * 64
+    torch.manual_seed(0)
+    qkv = (torch.randn(B * N, 3 * C, device="cuda") * 1.5).bfloat16()
+    th = ops.relpos_table_bf16(torch.randn(2 * h - 1, 64, device="cuda") * 0.3)
+    tw = ops.relpos_table_bf16(torch.randn(2 * w - 1, 64, device="cuda") * 0.3)
+    dout = (torch.randn(B * N, C, device="cuda") * 0.5).bfloat16()
+
+    def fwd():
+        return ops.attn_fwd(qkv, th, tw, B, heads, h, w, save_rel=True)
+
+    out, lse, rel = fwd()
+
+    def bwd():
+        return ops.attn_bwd(qkv, out, dout, lse, th, tw, B, heads, h, w, rel=rel)
+
+    dqkv, dTh, dTw = bwd()
+    if dump:
+        torch.save({"out": out.cpu(), "lse": lse.cpu(), "dqkv": dqkv.cpu(), "dTh": dTh.cpu(), "dTw": dTw.cpu()}, dump)
+
+    def timed(fn):
+        for _ in range(5):
+            fn()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(iters):
+            fn()
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / iters
+
+    fwd_ms, bwd_ms = timed(fwd), timed(bwd)
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(10):
+            bwd()
+        torch.cuda.synchronize()
+    kern = {}
+    for ev in prof.key_averages():
+        if ev.device_type == torch.autograd.DeviceType.CUDA and "attn" in ev.key:
+            kern[ev.key] = kern.get(ev.key, 0.0) + ev.device_time_total
+    tot = sum(kern.values()) or 1.0
+    ff, bf = attn_flops(B, heads, h, w)
+    return {"geom": name, "fwd_ms": round(fwd_ms, 4), "bwd_ms": round(bwd_ms, 4),
+            "fwd_bwd_ms": round(fwd_ms + bwd_ms, 4), "fwd_tflops": round(ff / fwd_ms / 1e9, 1),
+            "bwd_tflops": round(bf / bwd_ms / 1e9, 1),
+            "bwd_kernel_share": {k: round(v / tot, 3) for k, v in sorted(kern.items(), key=lambda kv: -kv[1])}}
+
+
+def compare_dumps(a, b):
+    import torch
+    x, y = torch.load(a), torch.load(b)
+    res = {}
+    for k in x:
+        d = (x[k].float() - y[k].float()).abs().max().item()
+        res[k] = d / max(x[k].float().abs().max().item(), 1e-9)
+    return res
+
+
+def run_bench(libs, rounds, iters):
+    """One JSON line per (round, geometry, library) on stdout; the operand dumps live in a temporary directory."""
+    import shutil
+    import tempfile
+    tmp = tempfile.mkdtemp(prefix="attn_bench_")
+    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True).stdout.strip()
+    print(json.dumps({"gpu": smi}), flush=True)
+    try:
+        for rnd in range(rounds):
+            for geom in [g[0] for g in BENCH_GEOMS]:
+                for i, lib in enumerate(libs):
+                    dump = os.path.join(tmp, f"{geom}_{i}.pt") if rnd == 0 else ""
+                    env = dict(os.environ, PK_LIB=os.path.abspath(lib))
+                    p = subprocess.run([sys.executable, __file__, "--bench-arm", geom, str(iters), dump], env=env,
+                                       capture_output=True, text=True, timeout=600)
+                    line = [l for l in p.stdout.splitlines() if l.startswith("RESULT ")]
+                    r = json.loads(line[-1][7:]) if line else {"geom": geom, "rc": p.returncode,
+                                                                "stderr": p.stderr[-1500:]}
+                    r.update(arm=lib, round=rnd)
+                    if dump and i > 0 and line:
+                        r["rel_diff_vs_arm0"] = compare_dumps(os.path.join(tmp, f"{geom}_0.pt"), dump)
+                    print(json.dumps(r), flush=True)
+    finally:
+        shutil.rmtree(tmp, ignore_errors=True)
+
+
 if __name__ == "__main__":
+    if len(sys.argv) >= 3 and sys.argv[1] == "--bench":
+        run_bench(sys.argv[2:], rounds=int(os.environ.get("ATTN_BENCH_ROUNDS", "2")),
+                  iters=int(os.environ.get("ATTN_BENCH_ITERS", "50")))
+        sys.exit(0)
+    if len(sys.argv) >= 5 and sys.argv[1] == "--bench-arm":
+        print("RESULT " + json.dumps(bench_arm(sys.argv[2], int(sys.argv[3]), sys.argv[4])), flush=True)
+        sys.exit(0)
     if len(sys.argv) >= 3 and sys.argv[1] == "--case":
         idx = int(sys.argv[2])
         try:
