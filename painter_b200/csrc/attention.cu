@@ -13,9 +13,13 @@
 //             domain, O += P V; writes O and the log-sum-exp.
 //   backward  dQ kernel (per 64 queries; also the bias-row gradients and the per-CTA table-gradient partials) and
 //             dK/dV kernel (per 64 keys, loops over the query tiles); both recompute P from the log-sum-exp.
-// The bias rows rel_h[q, i] = q . T_h[i_q - i + h - 1] and rel_w[q, j] = q . T_w[j_q - j + w - 1] (h + w dot products
-// per query, ~3 % of the attention FLOPs) are computed once per query tile on the FMA pipe and kept, log2e-scaled, in
-// shared memory; the training forward stores them for the backward kernels ([B*heads, Np, h] / [B*heads, Np, w]).
+// The bias rows rel_h[q, i] = q . T_h[i_q - i + h - 1] and rel_w[q, j] = q . T_w[j_q - j + w - 1] are one product
+// R = Q [T_h; T_w]^T per query tile (the tables staged as [rows][64] tiles), scattered from the accumulator into
+// log2e-scaled rows in shared memory; the training forward stores them for the backward kernels
+// ([B*heads, Np, h] / [B*heads, Np, w]).  The dQ kernel gets the bias-row gradients of each key tile as one more
+// product, dS . E with E the tile's one-hot [key][image column | image row] matrix, and its tail runs both table
+// terms as products over the Toeplitz matrix G[q, table row] of those gradients: dQ += G [T_h; T_w] and the
+// table-gradient partials G^T Q.
 #include "common.cuh"
 #include "wgmma.cuh"
 #include "host_common.h"
@@ -26,8 +30,6 @@ namespace pk {
 constexpr int AT_BM = 64;                     // rows (queries or keys) per CTA and per loop tile
 constexpr int AT_THREADS = 128;               // one warpgroup
 constexpr int AT_TILE = AT_BM * 128;          // bytes of one 64 x 64 bf16 operand tile
-constexpr int AT_TLD = 72;                    // bf16 per staged rel-pos table row (64 + 8 pad, FMA-pipe reads)
-constexpr int AT_DSLD = 65;                   // fp32 per row of the dQ kernel's dS tile (odd: conflict-free row reads)
 constexpr float AT_LOG2E = 1.4426950408889634f;
 
 struct AttnArgs {
@@ -52,9 +54,6 @@ __device__ __forceinline__ float bf16hi(uint32_t u) { return __uint_as_float(u &
 // Byte offset of 16-byte chunk `ch` of row `row` in a [rows][64] bf16 tile with 128-byte swizzle (8-row atoms of
 // 1024 bytes; the tile is 1024-byte aligned), the layout SWIZZLE_128B descriptors expect.
 __device__ __forceinline__ uint32_t sw128(int row, int ch) { return row * 128 + ((ch ^ (row & 7)) << 4); }
-__device__ __forceinline__ float sw128_elem(const uint8_t* tile, int row, int col) {
-  return __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(tile + sw128(row, col >> 3) + (col & 7) * 2));
-}
 
 // cp.async with zero fill: the destination gets `bytes` bytes from src and zeros for the rest of the copy size
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t bytes) {
@@ -94,12 +93,12 @@ __device__ __forceinline__ void mma_ss(float (&d)[32], uint32_t sa, uint32_t sb)
   for (int k = 0; k < 4; ++k)
     wgmma_m64n64k16<0, 0>(d, wgmma_desc_add(da, k * 32), wgmma_desc_add(db, k * 32), k > 0 ? 1u : 0u);
 }
-// d[64 x 64] += P . B: P as packed register fragments (pack_frag), B a [64][64] tile (rows = the reduction index)
-// read MN-major.
-__device__ __forceinline__ void mma_rs(float (&d)[32], const uint32_t (&p)[4][4], uint32_t sb) {
+// d[64 x 64] (+)= P . B: P as packed register fragments (pack_frag), B a [64][64] tile (rows = the reduction index)
+// read MN-major.  acc = 0 overwrites d.
+__device__ __forceinline__ void mma_rs(float (&d)[32], const uint32_t (&p)[4][4], uint32_t sb, uint32_t acc = 1u) {
   const uint64_t db = make_wgmma_desc(sb, AT_TILE, 1024);
 #pragma unroll
-  for (int k = 0; k < 4; ++k) wgmma_m64n64k16_rs<1>(d, p[k], wgmma_desc_add(db, k * 2048), 1u);
+  for (int k = 0; k < 4; ++k) wgmma_m64n64k16_rs<1>(d, p[k], wgmma_desc_add(db, k * 2048), k > 0 ? 1u : acc);
 }
 // accumulator fragment -> bf16 A fragments of the next product (wgmma_m64n64k16_rs)
 __device__ __forceinline__ void pack_frag(const float (&s)[32], uint32_t (&p)[4][4]) {
@@ -117,55 +116,99 @@ __device__ __forceinline__ void zero32(float (&d)[32]) {
   for (int i = 0; i < 32; ++i) d[i] = 0.f;
 }
 
-// Stage both bf16 tables (row stride AT_TLD) into sT.
-__device__ __forceinline__ void stage_tables(const AttnArgs& a, __nv_bfloat16* sT) {
-  const int Lh = 2 * a.h - 1, Lw = 2 * a.w - 1;
-  for (int idx = threadIdx.x; idx < (Lh + Lw) * 8; idx += AT_THREADS) {
+// Staged tables: one swizzled [rows][64] block, T_h in rows [0, tab_h_rows(h)), T_w in the next tab_h_rows(w) rows,
+// each zero past its 2h - 1 (2w - 1) real rows, the whole rounded up to 64 rows.  Read K-major in 64-row chunks by the
+// bias-row product (table rows = output columns) and MN-major by the dQ tail (table rows = the reduction index).
+__host__ __device__ inline int tab_h_rows(int h) { return (2 * h - 1 + 15) / 16 * 16; }
+__host__ __device__ inline int tab_rows(int h, int w) { return tab_h_rows(h) + tab_h_rows(w); }
+__host__ __device__ inline size_t table_bytes(int h, int w) { return static_cast<size_t>(tab_rows(h, w) + 63) / 64 * AT_TILE; }
+
+// Start copying both tables into the staged block at shared address s.
+__device__ __forceinline__ void load_tables(const AttnArgs& a, uint32_t s) {
+  const int Lh = 2 * a.h - 1, Lw = 2 * a.w - 1, hp = tab_h_rows(a.h);
+  const int rows = static_cast<int>(table_bytes(a.h, a.w) / 128);
+  for (int idx = threadIdx.x; idx < rows * 8; idx += AT_THREADS) {
     const int row = idx >> 3, ch = idx & 7;
-    const __nv_bfloat16* src = row < Lh ? a.th + static_cast<size_t>(row) * 64 : a.tw + static_cast<size_t>(row - Lh) * 64;
-    *reinterpret_cast<uint4*>(sT + row * AT_TLD + ch * 8) = *reinterpret_cast<const uint4*>(src + ch * 8);
+    const bool hs = row < hp;
+    const int tr = hs ? row : row - hp;
+    const bool valid = tr < (hs ? Lh : Lw);
+    const __nv_bfloat16* src = (hs ? a.th : a.tw) + static_cast<size_t>(valid ? tr : 0) * 64 + ch * 8;
+    cp_async16(s + sw128(row, ch), src, valid ? 16u : 0u);
   }
 }
 
 // Bias rows of the 64 queries [q0, q0 + 64) of one (batch, head), log2e-scaled, into relh_s [64][h] / relw_s [64][w]
-// (and to global when relh_g / relw_g are given).  sQ: the swizzled query tile; sT: scratch for both bf16 tables.
-__device__ void compute_bias_rows(const AttnArgs& a, const uint8_t* sQ, __nv_bfloat16* sT, int q0,
-                                  float* relh_s, float* relw_s, float* relh_g, float* relw_g) {
-  const int h = a.h, w = a.w, Lh = 2 * h - 1;
-  stage_tables(a, sT);
-  __syncthreads();
-  for (int idx = threadIdx.x; idx < AT_BM * (h + w); idx += AT_THREADS) {
-    const int q = idx / (h + w), k = idx - q * (h + w);
-    const int t = min(q0 + q, a.N - 1);
-    const int iq = t / w, jq = t - iq * w;
-    const int trow = k < h ? iq - k + h - 1 : Lh + jq - (k - h) + w - 1;
-    const uint4* qa = reinterpret_cast<const uint4*>(sQ + q * 128);
-    const uint32_t* ta = reinterpret_cast<const uint32_t*>(sT + trow * AT_TLD);
-    float s0 = 0.f, s1 = 0.f;
+// (and to global when relh_g / relw_g are given).  sQ: the query tile (its cp.async group committed); sT: scratch for
+// the staged tables.  R = Q . [T_h; T_w]^T in 64-column chunks; R[q, r] is rel_h[q, i_q + h - 1 - r] for the T_h rows
+// and rel_w[q, j_q + w - 1 - r'] for the T_w rows, so each (q, i) and (q, j) comes from exactly one accumulator entry.
+// Queries past N take the image position of query N - 1 (their Q rows are zero, so their rows are zero).
+__device__ void compute_bias_rows(const AttnArgs& a, uint32_t sQ, uint32_t sT, int q0, float* relh_s, float* relw_s,
+                                  float* relh_g, float* relw_g) {
+  const int h = a.h, w = a.w, hp = tab_h_rows(h), rows = tab_rows(h, w);
+  load_tables(a, sT);
+  cp_async_commit();
+  tiles_ready<0>();
+  const int lane = threadIdx.x & 31, c2 = 2 * (lane & 3);
+  const int rl0 = (threadIdx.x >> 5) * 16 + (lane >> 2);
+  int iq[2], jq[2];
 #pragma unroll
-    for (int ch = 0; ch < 8; ++ch) {
-      const uint4 x4 = qa[ch ^ (q & 7)];
-      const uint32_t x[4] = {x4.x, x4.y, x4.z, x4.w};
+  for (int e = 0; e < 2; ++e) {
+    const int t = min(q0 + rl0 + 8 * e, a.N - 1);
+    iq[e] = t / w;
+    jq[e] = t - iq[e] * w;
+  }
+  float r[32];
+  zero32(r);
+  for (int n0 = 0; n0 < rows; n0 += AT_BM) {
+    wgmma_fence_operands(r);
+    wgmma_fence();
+    mma_ss(r, sQ, sT + n0 * 128);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operands(r);
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const uint32_t y = ta[ch * 4 + e];
-        s0 = fmaf(bf16lo(x[e]), bf16lo(y), s0);
-        s1 = fmaf(bf16hi(x[e]), bf16hi(y), s1);
+    for (int i = 0; i < 32; ++i) {
+      const int e = (i >> 1) & 1, q = rl0 + 8 * e, col = n0 + 8 * (i >> 2) + c2 + (i & 1);
+      const float v = r[i] * AT_LOG2E;
+      if (col < hp) {
+        const int k = iq[e] + h - 1 - col;
+        if (k >= 0 && k < h) relh_s[q * h + k] = v;
+      } else {
+        const int k = jq[e] + w - 1 - (col - hp);
+        if (k >= 0 && k < w) relw_s[q * w + k] = v;
       }
     }
-    const float v = (s0 + s1) * AT_LOG2E;
-    if (k < h) {
-      relh_s[q * h + k] = v;
-      if (relh_g) relh_g[static_cast<size_t>(q0 + q) * h + k] = v;
-    } else {
-      relw_s[q * w + k - h] = v;
-      if (relw_g) relw_g[static_cast<size_t>(q0 + q) * w + k - h] = v;
+  }
+  if (relh_g) {
+    __syncthreads();
+    for (int i = threadIdx.x; i < AT_BM * h; i += AT_THREADS) relh_g[static_cast<size_t>(q0) * h + i] = relh_s[i];
+    for (int i = threadIdx.x; i < AT_BM * w; i += AT_THREADS) relw_g[static_cast<size_t>(q0) * w + i] = relw_s[i];
+  }
+}
+
+// Image (row, column) of the 16 key columns nt * 8 + c2 + u (u = 0, 1) a thread holds in every 64-key tile: set for
+// the first tile, then moved on by 64 keys per tile, so the score loops divide by w only once.
+__device__ __forceinline__ void key_coords_init(int c2, int w, int (&kr)[16], int (&kc)[16]) {
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int x = (j >> 1) * 8 + c2 + (j & 1);
+    kr[j] = x / w;
+    kc[j] = x - kr[j] * w;
+  }
+}
+__device__ __forceinline__ void key_coords_next(int dr, int dc, int w, int (&kr)[16], int (&kc)[16]) {
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    kr[j] += dr;
+    kc[j] += dc;
+    if (kc[j] >= w) {
+      kc[j] -= w;
+      ++kr[j];
     }
   }
 }
 
 // Shared-memory carve-ups (bytes past the 1024-byte aligned base; the launch adds 1024 bytes of alignment slack).
-__host__ __device__ inline size_t table_bytes(int h, int w) { return static_cast<size_t>(2 * h - 1 + 2 * w - 1) * AT_TLD * 2; }
 // forward / dQ: 2-stage K | V ring, which also holds the staged tables when no tile is in flight
 __host__ __device__ inline size_t kv_ring_bytes(int h, int w) {
   const size_t t = table_bytes(h, w);
@@ -192,7 +235,6 @@ attn_fwd_kernel(const AttnArgs a) {
   uint8_t* sm = aligned_smem(smem_raw, sQ);
   const uint32_t ring = sQ + AT_TILE;
   const int h = a.h, w = a.w, N = a.N, C = a.heads * 64;
-  __nv_bfloat16* sT = reinterpret_cast<__nv_bfloat16*>(sm + AT_TILE);
   float* relh_s = reinterpret_cast<float*>(sm + AT_TILE + kv_ring_bytes(h, w));
   float* relw_s = relh_s + AT_BM * h;
   const int q0 = blockIdx.x * AT_BM, head = blockIdx.y, b = blockIdx.z;
@@ -203,9 +245,7 @@ attn_fwd_kernel(const AttnArgs a) {
 
   load_tile(sQ, base, 3 * C, q0, N, head * 64);
   cp_async_commit();
-  cp_async_wait<0>();
-  __syncthreads();
-  compute_bias_rows(a, sm, sT, q0, relh_s, relw_s, a.relh ? a.relh + bh * a.Np * h : nullptr,
+  compute_bias_rows(a, sQ, ring, q0, relh_s, relw_s, a.relh ? a.relh + bh * a.Np * h : nullptr,
                     a.relw ? a.relw + bh * a.Np * w : nullptr);
   __syncthreads();   // the tables are dead: the ring takes their place
 
@@ -223,6 +263,9 @@ attn_fwd_kernel(const AttnArgs a) {
   const int lane = threadIdx.x & 31, g = lane >> 2, c2 = 2 * (lane & 3);
   const int rl0 = (threadIdx.x >> 5) * 16 + g;     // local query rows rl0, rl0 + 8
   const float sc = a.scale_log2;
+  const int dr = AT_BM / w, dc = AT_BM - dr * w;
+  int kr[16], kc[16];
+  key_coords_init(c2, w, kr, kc);
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   float o[32], s[32];
   zero32(o);
@@ -245,11 +288,9 @@ attn_fwd_kernel(const AttnArgs a) {
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         const int key = k0 + nt * 8 + c2 + (e & 1), r = rl0 + 8 * (e >> 1);
+        const int j = 2 * nt + (e & 1);
         float v = -INFINITY;
-        if (key < N) {
-          const int kr = key / w, kc = key - kr * w;
-          v = fmaf(s[4 * nt + e], sc, relh_s[r * h + kr] + relw_s[r * w + kc]);
-        }
+        if (key < N) v = fmaf(s[4 * nt + e], sc, relh_s[r * h + kr[j]] + relw_s[r * w + kc[j]]);
         s[4 * nt + e] = v;
         mx[e >> 1] = fmaxf(mx[e >> 1], v);
       }
@@ -278,6 +319,7 @@ attn_fwd_kernel(const AttnArgs a) {
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_operands(o);
+    key_coords_next(dr, dc, w, kr, kc);
     __syncthreads();   // stage t & 1 is free for tile t + 2
   }
 #pragma unroll
@@ -307,7 +349,6 @@ attn_bias_rows_kernel(const AttnArgs a) {
   uint32_t sQ;
   uint8_t* sm = aligned_smem(smem_raw, sQ);
   const int h = a.h, w = a.w, N = a.N, C = a.heads * 64;
-  __nv_bfloat16* sT = reinterpret_cast<__nv_bfloat16*>(sm + AT_TILE);
   float* relh_s = reinterpret_cast<float*>(sm + AT_TILE + table_bytes(h, w));
   float* relw_s = relh_s + AT_BM * h;
   const int q0 = blockIdx.x * AT_BM, head = blockIdx.y, b = blockIdx.z;
@@ -316,31 +357,31 @@ attn_bias_rows_kernel(const AttnArgs a) {
   pdl_wait();
   load_tile(sQ, a.qkv + static_cast<size_t>(b) * N * 3 * C, 3 * C, q0, N, head * 64);
   cp_async_commit();
-  cp_async_wait<0>();
-  __syncthreads();
-  compute_bias_rows(a, sm, sT, q0, relh_s, relw_s, a.relh + bh * a.Np * h, a.relw + bh * a.Np * w);
+  compute_bias_rows(a, sQ, sQ + AT_TILE, q0, relh_s, relw_s, a.relh + bh * a.Np * h, a.relw + bh * a.Np * w);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
 // backward, dQ side.  grid (query tiles, heads, B)
-//   dS = P * (dP - delta),  dQ = scale dS K + dRelh . T_h(gathered) + dRelw . T_w(gathered)
-//   dRelh[q, i] = sum of dS over the keys of image row i, dRelw[q, j] over image column j (each key tile's dS goes
-//   through shared memory and is summed by the owner threads of the row)
-//   table-gradient partials: ws[cta][c][r] = sum_q dRel[q, .] q[c] over the (q, bias column) pairs hitting table row r
-// smem: sQ | sdO | K/V ring (tables after the loop) | relh_s | relw_s | drelh_s | drelw_s | ds_s [64][AT_DSLD]
+//   dS = P * (dP - delta),  dQ = scale dS K + G [T_h; T_w]
+//   dRelh[q, i] = sum of dS over the keys of image row i, dRelw[q, j] over image column j: per key tile the product
+//   dS . E with the one-hot E[key x][column] = 1 at column (k0 + x) mod w and at column w + (k0 mod w + x) / w (image
+//   row k0 / w + that offset).  w <= 56 (attn_check) keeps w plus the tile's image rows within 64 columns; for w = 1
+//   the column part is left out and dRelw is the row sum of dRelh.  Each accumulator entry has one owner thread that
+//   adds it into drelh_s / drelw_s, tile after tile: no atomics, a fixed order, reproducible.
+//   G[q, r] = dRelh[q, i_q + h - 1 - r] for the T_h rows r of the staged tables (zero outside [0, h)), likewise for
+//   T_w; the table-gradient partials of the CTA are G^T Q, ws[cta][c][table row].
+// smem: sQ | sdO | K/V ring (tables after the loop) | E | relh_s | relw_s | drelh_s | drelw_s
 __global__ void __launch_bounds__(AT_THREADS)
 attn_bwd_dq_kernel(const AttnArgs a) {
   extern __shared__ uint8_t smem_raw[];
   uint32_t sQ;
   uint8_t* sm = aligned_smem(smem_raw, sQ);
-  const uint32_t sdO = sQ + AT_TILE, ring = sdO + AT_TILE;
+  const uint32_t sdO = sQ + AT_TILE, ring = sdO + AT_TILE, sE = ring + static_cast<uint32_t>(kv_ring_bytes(a.h, a.w));
   const int h = a.h, w = a.w, N = a.N, C = a.heads * 64, Lh = 2 * h - 1, Lw = 2 * w - 1;
-  __nv_bfloat16* sT = reinterpret_cast<__nv_bfloat16*>(sm + 2 * AT_TILE);
-  float* relh_s = reinterpret_cast<float*>(sm + 2 * AT_TILE + kv_ring_bytes(h, w));
+  float* relh_s = reinterpret_cast<float*>(sm + (sE - sQ) + AT_TILE);
   float* relw_s = relh_s + AT_BM * h;
   float* drelh_s = relw_s + AT_BM * w;
   float* drelw_s = drelh_s + AT_BM * h;
-  float* ds_s = drelw_s + AT_BM * w;
   const int q0 = blockIdx.x * AT_BM, head = blockIdx.y, b = blockIdx.z;
   const size_t bh = static_cast<size_t>(b) * a.heads + head;
   const __nv_bfloat16* base = a.qkv + static_cast<size_t>(b) * N * 3 * C;
@@ -375,8 +416,12 @@ attn_bwd_dq_kernel(const AttnArgs a) {
 
   const int lane = threadIdx.x & 31, g = lane >> 2, c2 = 2 * (lane & 3);
   const int rl0 = (threadIdx.x >> 5) * 16 + g;
-  const int own_r = threadIdx.x >> 1, part = threadIdx.x & 1;   // a row of this thread's own warp
   const float sc = a.scale_log2;
+  const int dr = AT_BM / w, dc = AT_BM - dr * w;
+  const int wcols = w > 1 ? w : 0;   // E columns [0, wcols): image columns; then image rows from k0 / w on
+  int kr[16], kc[16];
+  key_coords_init(c2, w, kr, kc);
+  int kr0 = 0, kc0 = 0;              // k0 / w, k0 mod w
   float lse[2], dlt[2];
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
@@ -391,6 +436,21 @@ attn_bwd_dq_kernel(const AttnArgs a) {
 
   for (int t = 0; t < ntiles; ++t) {
     issue(t + 1);
+    // E of this tile (the previous tile's products that read it have completed)
+#pragma unroll
+    for (int it = 0; it < (AT_BM * 8) / AT_THREADS; ++it) {
+      const int x = it * (AT_THREADS / 8) + (threadIdx.x >> 3), ch = threadIdx.x & 7;
+      const int xr = kc0 + x, rofs = xr / w;
+      const int ccol = w > 1 ? xr - rofs * w : -1, rcol = wcols + rofs;
+      uint32_t v[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const int c = ch * 8 + 2 * u;
+        v[u] = (c == ccol || c == rcol ? 0x3F80u : 0u) | (c + 1 == ccol || c + 1 == rcol ? 0x3F800000u : 0u);
+      }
+      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sE + sw128(x, ch)), "r"(v[0]), "r"(v[1]),
+                   "r"(v[2]), "r"(v[3]) : "memory");
+    }
     tiles_ready<1>();
     const uint32_t sK = ring + (t & 1) * 2 * AT_TILE, sV = sK + AT_TILE;
     const int k0 = t * AT_BM;
@@ -407,117 +467,139 @@ attn_bwd_dq_kernel(const AttnArgs a) {
     for (int nt = 0; nt < 8; ++nt)
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const int key = k0 + nt * 8 + c2 + (e & 1), r = rl0 + 8 * (e >> 1);
+        const int key = k0 + nt * 8 + c2 + (e & 1), r = rl0 + 8 * (e >> 1), j = 2 * nt + (e & 1);
         float ds = 0.f;
         if (key < N) {
-          const int kr = key / w, kc = key - kr * w;
-          const float p = fast_exp2(fmaf(s[4 * nt + e], sc, relh_s[r * h + kr] + relw_s[r * w + kc]) - lse[e >> 1]);
+          const float p = fast_exp2(fmaf(s[4 * nt + e], sc, relh_s[r * h + kr[j]] + relw_s[r * w + kc[j]]) - lse[e >> 1]);
           ds = p * (dp[4 * nt + e] - dlt[e >> 1]);
         }
         s[4 * nt + e] = ds;
-        ds_s[r * AT_DSLD + nt * 8 + c2 + (e & 1)] = ds;
       }
     uint32_t da[4][4];
     pack_frag(s, da);
-    __syncwarp();   // the warp's 16 rows of dS are in ds_s
-    {
-      // bias-row gradients: thread pair (2 own_r, 2 own_r + 1) owns row own_r of the warp's rows; the even thread
-      // takes the even image columns / key-tile image rows, the odd one the odd ones.  Every (row, column) has one
-      // owner, so plain adds in a fixed order: deterministic, no atomics.
-      const float* dsr = ds_s + own_r * AT_DSLD;
-      const int xn = min(AT_BM, N - k0), k0m = k0 % w, kr0 = k0 / w;
-      float* drw = drelw_s + own_r * w;
-      for (int c = part; c < w; c += 2) {
-        int x = c - k0m;
-        if (x < 0) x += w;
-        float acc = 0.f;
-        for (; x < xn; x += w) acc += dsr[x];
-        drw[c] += acc;
-      }
-      float* drh = drelh_s + own_r * h;
-      const int nslots = (k0 + xn - 1) / w - kr0 + 1;
-      for (int j = part; j < nslots; j += 2) {
-        const int xa = max(0, (kr0 + j) * w - k0), xb = min(xn, (kr0 + j + 1) * w - k0);
-        float acc = 0.f;
-        for (int x = xa; x < xb; ++x) acc += dsr[x];
-        drh[kr0 + j] += acc;
-      }
-    }
+    // dQ += dS . K and, into s, this tile's bias-row gradients dS . E
     wgmma_fence_operands(dq);
+    wgmma_fence_operands(s);
     wgmma_fence();
     mma_rs(dq, da, sK);
+    mma_rs(s, da, sE, 0u);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_operands(dq);
-    __syncthreads();   // stage t & 1 is free for tile t + 2
+    wgmma_fence_operands(s);
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const int r = rl0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + c2 + (i & 1);
+      if (col < wcols) {
+        drelw_s[r * w + col] += s[i];
+      } else {
+        const int ir = kr0 + col - wcols;
+        if (ir < h) drelh_s[r * h + ir] += s[i];
+      }
+    }
+    key_coords_next(dr, dc, w, kr, kc);
+    kr0 += dr;
+    kc0 += dc;
+    if (kc0 >= w) {
+      kc0 -= w;
+      ++kr0;
+    }
+    __syncthreads();   // stage t & 1 is free for tile t + 2, E for tile t + 1
   }
-  cp_async_wait<0>();
-  stage_tables(a, sT);
-  __syncthreads();   // tables staged, drelh_s / drelw_s complete
+  load_tables(a, ring);
+  cp_async_commit();
+  if (w == 1 && threadIdx.x < AT_BM) {
+    float acc = 0.f;
+    for (int k = 0; k < h; ++k) acc += drelh_s[threadIdx.x * h + k];
+    drelw_s[threadIdx.x] = acc;
+  }
+  tiles_ready<0>();   // tables staged, drelh_s / drelw_s complete
 
-  // dQ = scale dS K + gathered table rows, written into the q columns of dqkv
+  // G[q, r] of the T_h rows (r < hp) and T_w rows of the staged tables; `q` local, `iq` / `jq` its image position
+  const int hp = tab_h_rows(h), krows = tab_rows(h, w);
+  auto gval = [&](int q, int iq, int jq, int r) -> float {
+    if (r < hp) {
+      const int k = iq + h - 1 - r;
+      return k >= 0 && k < h ? drelh_s[q * h + k] : 0.f;
+    }
+    const int k = jq + w - 1 - (r - hp);
+    return k >= 0 && k < w ? drelw_s[q * w + k] : 0.f;
+  };
+
+  // dQ = (dS K + 8 G [T_h; T_w]) / 8, written into the q columns of dqkv (G stored times 8: exact in bf16)
+  {
+    int iq[2], jq[2];
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int tq = min(q0 + rl0 + 8 * e, N - 1);
+      iq[e] = tq / w;
+      jq[e] = tq - iq[e] * w;
+    }
+    const uint64_t dt = make_wgmma_desc(ring, AT_TILE, 1024);
+    wgmma_fence_operands(dq);
+    for (int kk = 0; kk < krows / 16; ++kk) {
+      uint32_t ga[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const int e = u & 1, q = rl0 + 8 * e, r = 16 * kk + 8 * (u >> 1) + c2;
+        ga[u] = pack_bf16x2(8.f * gval(q, iq[e], jq[e], r), 8.f * gval(q, iq[e], jq[e], r + 1));
+      }
+      wgmma_fence();
+      wgmma_m64n64k16_rs<1>(dq, ga, wgmma_desc_add(dt, kk * 2048), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operands(dq);
+  }
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
-    const int r = rl0 + 8 * i, t = q0 + r;
-    const int tc = min(t, N - 1), iq = tc / w, jq = tc - iq * w;
-    float acc[16];
-#pragma unroll
-    for (int dt = 0; dt < 8; ++dt) {
-      acc[2 * dt] = dq[4 * dt + 2 * i] * 0.125f;
-      acc[2 * dt + 1] = dq[4 * dt + 2 * i + 1] * 0.125f;
-    }
-    for (int k = 0; k < h; ++k) {
-      const float d = drelh_s[r * h + k];
-      const __nv_bfloat16* trow = sT + (iq - k + h - 1) * AT_TLD + c2;
-#pragma unroll
-      for (int dt = 0; dt < 8; ++dt) {
-        const uint32_t u = *reinterpret_cast<const uint32_t*>(trow + dt * 8);
-        acc[2 * dt] = fmaf(d, bf16lo(u), acc[2 * dt]);
-        acc[2 * dt + 1] = fmaf(d, bf16hi(u), acc[2 * dt + 1]);
-      }
-    }
-    for (int k = 0; k < w; ++k) {
-      const float d = drelw_s[r * w + k];
-      const __nv_bfloat16* trow = sT + (Lh + jq - k + w - 1) * AT_TLD + c2;
-#pragma unroll
-      for (int dt = 0; dt < 8; ++dt) {
-        const uint32_t u = *reinterpret_cast<const uint32_t*>(trow + dt * 8);
-        acc[2 * dt] = fmaf(d, bf16lo(u), acc[2 * dt]);
-        acc[2 * dt + 1] = fmaf(d, bf16hi(u), acc[2 * dt + 1]);
-      }
-    }
+    const int t = q0 + rl0 + 8 * i;
     if (t < N) {
       __nv_bfloat16* drow = a.out + (static_cast<size_t>(b) * N + t) * 3 * C + head * 64;
 #pragma unroll
       for (int dt = 0; dt < 8; ++dt)
-        *reinterpret_cast<uint32_t*>(drow + dt * 8 + c2) = pack_bf16x2(acc[2 * dt], acc[2 * dt + 1]);
+        *reinterpret_cast<uint32_t*>(drow + dt * 8 + c2) =
+            pack_bf16x2(dq[4 * dt + 2 * i] * 0.125f, dq[4 * dt + 2 * i + 1] * 0.125f);
     }
   }
 
-  // table-gradient partials of this CTA (every entry of the slice is written)
+  // table-gradient partials of this CTA, G^T Q in 64-row chunks of the staged table rows (every entry of the slice
+  // is written; queries past N contribute nothing)
   const int rows = Lh + Lw;
   float* ws = a.dt_ws + ((bh * gridDim.x) + blockIdx.x) * static_cast<size_t>(rows) * 64;
-  // Only the queries whose bias column hits table row r contribute: per image row ir of the tile, table row r < Lh
-  // takes column i = ir + h - 1 - r of every query in that image row, and table row Lh + rw takes column
-  // j = jq + w - 1 - rw of the queries with jq in [rw - w + 1, rw]; both are contiguous query ranges.
-  const int qn = min(AT_BM, N - q0);
-  const int ir0 = q0 / w, ir1 = (q0 + qn - 1) / w;
-  for (int idx = threadIdx.x; idx < rows * 64; idx += AT_THREADS) {
-    const int c = idx / rows, r = idx - c * rows;
-    float acc = 0.f;
-    for (int ir = ir0; ir <= ir1; ++ir) {
-      const int ta = max(q0, ir * w), tb = min(q0 + qn, (ir + 1) * w);
-      if (r < Lh) {
-        const int i = ir + h - 1 - r;
-        if (i < 0 || i >= h) continue;
-        for (int t = ta; t < tb; ++t) acc = fmaf(drelh_s[(t - q0) * h + i], sw128_elem(sm, t - q0, c), acc);
-      } else {
-        const int rw = r - Lh, jofs = w - 1 - rw - ir * w;   // j = t + jofs
-        for (int t = max(ta, ir * w + rw - w + 1); t < min(tb, ir * w + rw + 1); ++t)
-          acc = fmaf(drelw_s[(t - q0) * w + t + jofs], sw128_elem(sm, t - q0, c), acc);
+  int qiq[16], qjq[16];   // image position of the queries 16 kk + 8 v + c2 + u of the A fragments, iq = -h if past N
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int tq = q0 + (j >> 2) * 16 + ((j >> 1) & 1) * 8 + c2 + (j & 1);
+    qiq[j] = tq < N ? tq / w : -h;
+    qjq[j] = tq < N ? tq - qiq[j] * w : -w;
+  }
+  const uint64_t dqd = make_wgmma_desc(sQ, AT_TILE, 1024);
+  float acc[32];
+  zero32(acc);
+  for (int m0 = 0; m0 < krows; m0 += AT_BM) {
+    uint32_t ga[4][4];
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const int r = m0 + rl0 + 8 * (u & 1), j = 4 * kk + 2 * (u >> 1), q = j >> 2 << 4 | ((j >> 1) & 1) << 3 | c2;
+        ga[kk][u] = pack_bf16x2(gval(q, qiq[j], qjq[j], r), gval(q + 1, qiq[j + 1], qjq[j + 1], r));
+        asm volatile("" : "+r"(ga[kk][u])::"memory");
       }
+    wgmma_fence_operands(acc);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_rs<1>(acc, ga[kk], wgmma_desc_add(dqd, kk * 2048), kk > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operands(acc);
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const int r = m0 + rl0 + 8 * ((i >> 1) & 1), c = 8 * (i >> 2) + c2 + (i & 1);
+      const int wr = r < hp ? (r < Lh ? r : -1) : (r - hp < Lw ? Lh + r - hp : -1);
+      if (wr >= 0) ws[static_cast<size_t>(c) * rows + wr] = acc[i];
     }
-    ws[idx] = acc;
   }
 }
 
@@ -821,7 +903,7 @@ static int attn_bwd_impl(const void* qkv, const void* O, const void* dO, const f
     PK_LAUNCH_CHECK("pk_attn_bwd(delta)");
   }
   if (launch_attn(attn_bwd_dq_kernel, grid,
-                  1024 + 2 * AT_TILE + kv_ring_bytes(h, w) + 2 * rel_bytes + AT_BM * AT_DSLD * 4, st, a,
+                  1024 + 3 * AT_TILE + kv_ring_bytes(h, w) + 2 * rel_bytes, st, a,
                   "pk_attn_bwd(dq)"))
     return 2;
   {

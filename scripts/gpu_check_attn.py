@@ -135,7 +135,8 @@ def _run_fwd_checks(res, qkv, th, tw, out, lse, B, heads, h, w):
         res["tflops"] = 4.0 * B * heads * N * N * 64 / ms / 1e9
 
 
-# Kernel-level timing of the training path (attn_fwd(save_rel=True) + attn_bwd(rel=...)) at the bench geometries.
+# Kernel-level timing at the bench geometries of the saved-rows pair (attn_fwd(save_rel=True) + attn_bwd(rel=...))
+# and of the pair the attention module runs (attn_fwd + attn_bwd, which recomputes the bias rows in its own kernel).
 # `--bench LIB [LIB ...]` times each library in its own process (PK_LIB selects it), alternating over
 # $ATTN_BENCH_ROUNDS rounds, and compares every arm's outputs with the first arm's on the same seeded operands.
 BENCH_GEOMS = [("train_b8", 8, 16, 56, 28), ("long_b2", 2, 16, 112, 56)]
@@ -182,22 +183,34 @@ def bench_arm(geom, iters, dump):
         torch.cuda.synchronize()
         return e0.elapsed_time(e1) / iters
 
+    def mod_fwd():
+        return ops.attn_fwd(qkv, th, tw, B, heads, h, w)
+
+    def mod_bwd():
+        return ops.attn_bwd(qkv, out, dout, lse, th, tw, B, heads, h, w)
+
     fwd_ms, bwd_ms = timed(fwd), timed(bwd)
-    from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for _ in range(10):
-            bwd()
-        torch.cuda.synchronize()
-    kern = {}
-    for ev in prof.key_averages():
-        if ev.device_type == torch.autograd.DeviceType.CUDA and "attn" in ev.key:
-            kern[ev.key] = kern.get(ev.key, 0.0) + ev.device_time_total
-    tot = sum(kern.values()) or 1.0
+    mod_fwd_ms, mod_bwd_ms = timed(mod_fwd), timed(mod_bwd)
+
+    def shares(fn):
+        from torch.profiler import ProfilerActivity, profile
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(10):
+                fn()
+            torch.cuda.synchronize()
+        kern = {}
+        for ev in prof.key_averages():
+            if ev.device_type == torch.autograd.DeviceType.CUDA and "attn" in ev.key:
+                kern[ev.key] = kern.get(ev.key, 0.0) + ev.device_time_total
+        tot = sum(kern.values()) or 1.0
+        return {k: round(v / tot, 3) for k, v in sorted(kern.items(), key=lambda kv: -kv[1])}
+
     ff, bf = attn_flops(B, heads, h, w)
     return {"geom": name, "fwd_ms": round(fwd_ms, 4), "bwd_ms": round(bwd_ms, 4),
             "fwd_bwd_ms": round(fwd_ms + bwd_ms, 4), "fwd_tflops": round(ff / fwd_ms / 1e9, 1),
-            "bwd_tflops": round(bf / bwd_ms / 1e9, 1),
-            "bwd_kernel_share": {k: round(v / tot, 3) for k, v in sorted(kern.items(), key=lambda kv: -kv[1])}}
+            "bwd_tflops": round(bf / bwd_ms / 1e9, 1), "bwd_kernel_share": shares(bwd),
+            "module_fwd_ms": round(mod_fwd_ms, 4), "module_bwd_ms": round(mod_bwd_ms, 4),
+            "module_fwd_bwd_ms": round(mod_fwd_ms + mod_bwd_ms, 4), "module_bwd_kernel_share": shares(mod_bwd)}
 
 
 def compare_dumps(a, b):
