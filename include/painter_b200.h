@@ -263,7 +263,11 @@ int pk_bilinear_u8(const double* seg, int SH, int SW, uint8_t* dst, int OH, int 
  *  pk_im2col_patch_split3    PatchEmbed im2col of imgs and tgts (vitdet_utils.py:178-186) as split A operand
  *  pk_dec_im2col_split3      pixel shuffle + 3x3 im2col of decoder_embed's output (models_painter.py:424-430)
  *  pk_head_f32               LayerNorm2D + exact GELU + conv1x1 + masked loss terms + patchify, fp32, from the fp32
- *                            conv3x3 output [B*H*W, 64]; num accumulates in fp64 (num_zeroed) and is emitted as fp32  */
+ *                            conv3x3 output [B*H*W, 64]; num accumulates in fp64 (num_zeroed) and is emitted as fp32
+ *  pk_attn_fwd_split3        fused attention with decomposed rel-pos bias in the same split arithmetic, without the
+ *                            score matrix: qkv fp32 [B*h*w, 3C] (the qkv GEMM's layout), th / tw fp32 [2h-1, 64] /
+ *                            [2w-1, 64] -> out fp32 [B*h*w, C] (heads merged).  h <= 112, w <= 56; a windowed block
+ *                            calls it with B = all windows and h = w = window size.  No allocation or host sync.  */
 int pk_split3(const float* x, int ldx, void* out_bf16, int M, int K, int side_b, int gelu, void* stream);
 int pk_split3_heads(const float* qkv, void* out_bf16, int B, int heads, int N, int Npad, int which, void* stream);
 int pk_softmax_relpos_split3(const float* S, const float* Gh, int ldgh, const float* Gw, int ldgw, void* P_bf16,
@@ -274,6 +278,8 @@ int pk_dec_im2col_split3(const float* D, void* out_bf16, int B, int h, int w, in
 int pk_head_f32(const float* c1, const float* head_params, const float* tgts, const uint8_t* mask, int maskB,
                 const float* valid, float* patch, double* num_zeroed, float* num_out, int B, int H, int W, int p,
                 int loss_kind, void* stream);
+int pk_attn_fwd_split3(const float* qkv, const float* th, const float* tw, float* out, int B, int heads, int h, int w,
+                       void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Training data path, per-sample device work (SURVEY §8 f.4).

@@ -8,9 +8,10 @@ Selected by `model.precision`:  "bf16" = the training arithmetic (bf16 tensor-co
 
 Still tensor-core code: every GEMM operand is split into three bf16 terms and the six significant cross products run as
 ONE pk_gemm_bf16 call over K-concatenated operands (csrc/accurate.cu has the derivation); softmax, LayerNorm, GELU
-(exact erf), the residual stream and the loss stay fp32 (the loss numerator accumulates in fp64).  Attention
-materialises the score matrix per (sample, head) like the reference does - this mode is about digits, not speed:
-6x the tensor-core work of the bf16 path plus the split passes.
+(exact erf), the residual stream and the loss stay fp32 (the loss numerator accumulates in fp64).  Global blocks
+materialise the score matrix per (sample, head) like the reference does (`attention`); windowed blocks run all their
+windows through one fused kernel in the same split arithmetic (ops.attn_fwd_split3) - this mode is about digits,
+not speed: 6x the tensor-core work of the bf16 path plus the split passes.
 
 Stage map = engine.py's (same reference lines): embed, 24 blocks (+ early merge, SegGPT ensemble), decoder, loss.
 """
@@ -112,20 +113,32 @@ def _split_table(t, L):
 
 
 def block(z, blk, Bp, h, w, heads, eps, ens, ws_cache, rel_h, rel_w):
-    """models_painter.py:216-235 (+ SegGPT ensemble models_seggpt.py:220-231); eval mode (DropPath = identity)."""
+    """models_painter.py:216-235 (+ SegGPT ensemble models_seggpt.py:220-231); eval mode (DropPath = identity).
+    rel_h / rel_w: the block's tables for its attention grid (the window for a windowed block)."""
     N = h * w
     C = z.shape[1]
-    if blk.window_size > 0:
-        raise NotImplementedError("painter_b200 fp32-accurate mode: windowed blocks are not implemented (no stock "
-                                  "configuration has any, SURVEY.md section 0.1)")
+    ws = blk.window_size
     u, _, _ = ops.layernorm_fwd(z, blk.norm1.weight, blk.norm1.bias, eps, out_dtype=torch.float32, want_stats=False)
-    ao = attention(u, blk, Bp, h, w, heads, ws_cache, rel_h, rel_w)
     a = blk.attn
-    if ens[0] > 0:
+    if ws > 0:
+        # vitdet_utils.py:16-60: LN1's output is zero-padded to whole windows BEFORE qkv, so padded tokens carry the qkv
+        # bias and take part as keys.  Partitioning the split operand is exact: zero rows split to zero.
+        us = ops.window_partition_bf16(split3(u), Bp, h, w, ws)
+        Bw = us.shape[0] // (ws * ws)
+        qkv = _gemm(us, split_weight(a.qkv.weight), kind=EPI_F32, bias=a.qkv.bias)
+        ao = ops.attn_fwd_split3(qkv, rel_h.detach().contiguous(), rel_w.detach().contiguous(), Bw, heads, ws, ws)
         pa = _gemm(split3(ao), split_weight(a.proj.weight), kind=EPI_F32, bias=a.proj.bias)
-        x1 = ops.ensemble_resid(pa, z, ens[0], ens[1], N, C)
+        if ens[0] > 0:   # the ensemble merges on the full token grid, after window_unpartition (models_seggpt.py:214-231)
+            x1 = ops.ensemble_resid(ops.window_unpartition(pa, Bp, h, w, ws), z, ens[0], ens[1], N, C)
+        else:
+            x1 = ops.window_unpartition(pa, Bp, h, w, ws, resid=z)
     else:
-        x1 = _gemm(split3(ao), split_weight(a.proj.weight), kind=EPI_RESID, bias=a.proj.bias, aux=z)
+        ao = attention(u, blk, Bp, h, w, heads, ws_cache, rel_h, rel_w)
+        if ens[0] > 0:
+            pa = _gemm(split3(ao), split_weight(a.proj.weight), kind=EPI_F32, bias=a.proj.bias)
+            x1 = ops.ensemble_resid(pa, z, ens[0], ens[1], N, C)
+        else:
+            x1 = _gemm(split3(ao), split_weight(a.proj.weight), kind=EPI_RESID, bias=a.proj.bias, aux=z)
     v, _, _ = ops.layernorm_fwd(x1, blk.norm2.weight, blk.norm2.bias, eps, out_dtype=torch.float32, want_stats=False)
     hid = _gemm(split3(v), split_weight(blk.mlp.fc1.weight), kind=EPI_F32, bias=blk.mlp.fc1.bias)
     return _gemm(split3(hid, gelu=True), split_weight(blk.mlp.fc2.weight), kind=EPI_RESID, bias=blk.mlp.fc2.bias, aux=x1)
@@ -162,8 +175,9 @@ def forward(model, imgs, tgts, mask_u8, valid, type_emb, merge_between_batch):
         ens = (0, 0)
         if merge_between_batch >= 0 and i >= merge_between_batch:
             ens = (2, B) if merge_idx >= i else (1, B)
-        rel_h = engine.resize_rel_table(blk.attn.rel_pos_h, h)
-        rel_w = engine.resize_rel_table(blk.attn.rel_pos_w, w)
+        ws = blk.window_size
+        rel_h = engine.resize_rel_table(blk.attn.rel_pos_h, ws if ws > 0 else h)
+        rel_w = engine.resize_rel_table(blk.attn.rel_pos_w, ws if ws > 0 else w)
         z = block(z, blk, Bp, h, w, model.num_heads, blk.norm1.eps, ens, ws_cache, rel_h, rel_w)
         if i == merge_idx:
             z = ops.merge_halves(z)

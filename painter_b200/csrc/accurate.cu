@@ -5,26 +5,18 @@
 //     h = bf16(x),  m = bf16(x - h),  l = bf16(x - h - m)          (x = h + m + l up to 2^-24 |x|)
 // and a product a.b is evaluated as  a_l b_h + a_m b_m + a_h b_l + a_m b_h + a_h b_m + a_h b_h  (the six terms above
 // 2^-24; smallest first) by CONCATENATING the terms along K:  A' = [l | m | h | m | h | h],  B' = [h | m | l | h | m | h],
-// K' = 6 K - ONE ordinary tcgen05 GEMM (pk_gemm_bf16) with fp32 accumulation in TMEM.  The kernels here produce those
-// split operands (fused with the elementwise step in front of the GEMM: GELU, softmax, im2col) and the few fp32
-// elementwise stages the bf16 path had fused into GEMM epilogues.  All are HBM-bound streaming kernels.
+// K' = 6 K - ONE ordinary wgmma GEMM (pk_gemm_bf16) with fp32 accumulation in registers.  The kernels here produce
+// those split operands (fused with the elementwise step in front of the GEMM: GELU, softmax, im2col) and the few fp32
+// elementwise stages the bf16 path had fused into GEMM epilogues.  All are HBM-bound streaming kernels.  The split
+// itself and the term order (split3.cuh) are shared with the fused split attention forward of windowed blocks
+// (pk_attn_fwd_split3, attention.cu), which splits its tiles in shared memory instead of writing 6x-wide operands.
 #include "common.cuh"
+#include "split3.cuh"
 #include "host_common.h"
 #include "../../include/painter_b200.h"
 
 namespace pk {
 
-// term index of K-block t (0..5) for an A-side / B-side operand: 0 = h, 1 = m, 2 = l
-__device__ __constant__ int c_termA[6] = {2, 1, 0, 1, 0, 0};
-__device__ __constant__ int c_termB[6] = {0, 1, 2, 0, 1, 0};
-
-__device__ __forceinline__ void split3(float x, __nv_bfloat16 (&t)[3]) {
-  t[0] = __float2bfloat16_rn(x);
-  const float r1 = x - __bfloat162float(t[0]);
-  t[1] = __float2bfloat16_rn(r1);
-  const float r2 = r1 - __bfloat162float(t[1]);
-  t[2] = __float2bfloat16_rn(r2);
-}
 __device__ __forceinline__ float gelu_exact(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
 
 static inline int stream_grid2(size_t total, int block = 256) {

@@ -1,4 +1,5 @@
-// painter_b200 — fused global attention with decomposed relative-position bias, forward and backward (sm_90a).
+// painter_b200 — fused attention with decomposed relative-position bias, forward and backward (sm_90a), and the
+// fp32-accurate forward of windowed blocks (attn_fwd_split3_kernel, below the bf16 forward).
 //
 // Replaces models_painter.py:73-86 + util/vitdet_utils.py:63-125 (q*scale @ k^T, add_decomposed_rel_pos, softmax,
 // @ v) and autograd's backward through them, without ever materialising the [B*heads, N, N] score tensor.
@@ -22,6 +23,7 @@
 // table-gradient partials G^T Q.
 #include "common.cuh"
 #include "wgmma.cuh"
+#include "split3.cuh"
 #include "host_common.h"
 #include "../../include/painter_b200.h"
 
@@ -86,12 +88,12 @@ __device__ __forceinline__ void tiles_ready() {
 }
 
 // d[64 x 64] = A . B^T: A a [64][64] tile (rows = output rows), B a [64][64] tile (rows = output columns), both
-// K-major.  Issues the wgmmas only; the caller fences, commits and waits.
-__device__ __forceinline__ void mma_ss(float (&d)[32], uint32_t sa, uint32_t sb) {
+// K-major.  Issues the wgmmas only; the caller fences, commits and waits.  acc = 1 adds to d.
+__device__ __forceinline__ void mma_ss(float (&d)[32], uint32_t sa, uint32_t sb, uint32_t acc = 0u) {
   const uint64_t da = make_wgmma_desc(sa, 16, 1024), db = make_wgmma_desc(sb, 16, 1024);
 #pragma unroll
   for (int k = 0; k < 4; ++k)
-    wgmma_m64n64k16<0, 0>(d, wgmma_desc_add(da, k * 32), wgmma_desc_add(db, k * 32), k > 0 ? 1u : 0u);
+    wgmma_m64n64k16<0, 0>(d, wgmma_desc_add(da, k * 32), wgmma_desc_add(db, k * 32), k > 0 ? 1u : acc);
 }
 // d[64 x 64] (+)= P . B: P as packed register fragments (pack_frag), B a [64][64] tile (rows = the reduction index)
 // read MN-major.  acc = 0 overwrites d.
@@ -137,23 +139,24 @@ __device__ __forceinline__ void load_tables(const AttnArgs& a, uint32_t s) {
   }
 }
 
-// Bias rows of the 64 queries [q0, q0 + 64) of one (batch, head), log2e-scaled, into relh_s [64][h] / relw_s [64][w]
-// (and to global when relh_g / relw_g are given).  sQ: the query tile (its cp.async group committed); sT: scratch for
-// the staged tables.  R = Q . [T_h; T_w]^T in 64-column chunks; R[q, r] is rel_h[q, i_q + h - 1 - r] for the T_h rows
-// and rel_w[q, j_q + w - 1 - r'] for the T_w rows, so each (q, i) and (q, j) comes from exactly one accumulator entry.
-// Queries past N take the image position of query N - 1 (their Q rows are zero, so their rows are zero).
-__device__ void compute_bias_rows(const AttnArgs& a, uint32_t sQ, uint32_t sT, int q0, float* relh_s, float* relw_s,
-                                  float* relh_g, float* relw_g) {
-  const int h = a.h, w = a.w, hp = tab_h_rows(h), rows = tab_rows(h, w);
-  load_tables(a, sT);
-  cp_async_commit();
-  tiles_ready<0>();
+// Bias rows of the 64 queries [q0, q0 + 64) of one (batch, head) into relh_s [64][h] / relw_s [64][w] from the query
+// tile sQ and the staged tables sT (both visible to wgmma).  R = Q . [T_h; T_w]^T in 64-column chunks; R[q, r] is
+// rel_h[q, i_q + h - 1 - r] for the T_h rows and rel_w[q, j_q + w - 1 - r'] for the T_w rows, so each (q, i) and
+// (q, j) comes from exactly one accumulator entry.  Queries past N take the image position of query N - 1 (their Q
+// rows are zero, so their rows are zero).
+//   SPLIT = false: bf16 operands, one product, rows scaled by log2e (the log2-domain softmax of the bf16 kernels).
+//   SPLIT = true:  three-term split operands (split3.cuh): sQ's terms AT_TILE bytes apart, sT's `tterm` bytes apart;
+//                  the six products in c_termA / c_termB order, rows unscaled.
+template <bool SPLIT>
+__device__ __forceinline__ void bias_rows_product(int h, int w, int N, uint32_t sQ, uint32_t sT, uint32_t tterm,
+                                                  int q0, float* relh_s, float* relw_s) {
+  const int hp = tab_h_rows(h), rows = tab_rows(h, w);
   const int lane = threadIdx.x & 31, c2 = 2 * (lane & 3);
   const int rl0 = (threadIdx.x >> 5) * 16 + (lane >> 2);
   int iq[2], jq[2];
 #pragma unroll
   for (int e = 0; e < 2; ++e) {
-    const int t = min(q0 + rl0 + 8 * e, a.N - 1);
+    const int t = min(q0 + rl0 + 8 * e, N - 1);
     iq[e] = t / w;
     jq[e] = t - iq[e] * w;
   }
@@ -162,14 +165,20 @@ __device__ void compute_bias_rows(const AttnArgs& a, uint32_t sQ, uint32_t sT, i
   for (int n0 = 0; n0 < rows; n0 += AT_BM) {
     wgmma_fence_operands(r);
     wgmma_fence();
-    mma_ss(r, sQ, sT + n0 * 128);
+    if constexpr (SPLIT) {
+#pragma unroll
+      for (int k = 0; k < 6; ++k)
+        mma_ss(r, sQ + c_termA[k] * AT_TILE, sT + c_termB[k] * tterm + n0 * 128, k > 0 ? 1u : 0u);
+    } else {
+      mma_ss(r, sQ, sT + n0 * 128);
+    }
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_operands(r);
 #pragma unroll
     for (int i = 0; i < 32; ++i) {
       const int e = (i >> 1) & 1, q = rl0 + 8 * e, col = n0 + 8 * (i >> 2) + c2 + (i & 1);
-      const float v = r[i] * AT_LOG2E;
+      const float v = SPLIT ? r[i] : r[i] * AT_LOG2E;
       if (col < hp) {
         const int k = iq[e] + h - 1 - col;
         if (k >= 0 && k < h) relh_s[q * h + k] = v;
@@ -179,6 +188,17 @@ __device__ void compute_bias_rows(const AttnArgs& a, uint32_t sQ, uint32_t sT, i
       }
     }
   }
+}
+
+// bf16 bias rows, log2e-scaled, into relh_s / relw_s (and to global when relh_g / relw_g are given).  sQ: the query
+// tile (its cp.async group committed); sT: scratch for the staged tables.
+__device__ void compute_bias_rows(const AttnArgs& a, uint32_t sQ, uint32_t sT, int q0, float* relh_s, float* relw_s,
+                                  float* relh_g, float* relw_g) {
+  const int h = a.h, w = a.w;
+  load_tables(a, sT);
+  cp_async_commit();
+  tiles_ready<0>();
+  bias_rows_product<false>(h, w, a.N, sQ, sT, 0, q0, relh_s, relw_s);
   if (relh_g) {
     __syncthreads();
     for (int i = threadIdx.x; i < AT_BM * h; i += AT_THREADS) relh_g[static_cast<size_t>(q0) * h + i] = relh_s[i];
@@ -358,6 +378,215 @@ attn_bias_rows_kernel(const AttnArgs a) {
   load_tile(sQ, a.qkv + static_cast<size_t>(b) * N * 3 * C, 3 * C, q0, N, head * 64);
   cp_async_commit();
   compute_bias_rows(a, sQ, sQ + AT_TILE, q0, relh_s, relw_s, a.relh + bh * a.Np * h, a.relw + bh * a.Np * w);
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// fp32-accurate forward (pk_attn_fwd_split3; the attention of windowed blocks in the fp32 inference mode).
+// grid (query tiles, heads, B).  The tiling, key streaming and online softmax of attn_fwd_kernel on fp32 operands:
+// every operand tile is staged as the three bf16 terms h, m, l of accurate.cu's split (split3.cuh), and each product is
+// the six terms above 2^-24 in c_termA / c_termB order, accumulated in fp32 by wgmma:
+//   S = sum_6 q_a k_b^T, R = sum_6 q_a [T_h; T_w]_b^T (bias rows), O += sum_6 p_a v_b (P split in registers).
+// S is taken on the unscaled q and multiplied by 0.125 in the softmax (a power of two: exactly the product on the
+// scaled q), so one split Q tile serves S and the bias rows, which the reference computes on the unscaled q.  The
+// softmax runs in the natural-log domain with expf.  K and V arrive as raw fp32 through cp.async one tile ahead and
+// are split in shared memory; Q and the tables are split on their way in.
+// smem: sQ (3 terms) | split K (3) | split V (3) | raw K | raw V (two tiles of 64 rows x 32 fp32 each; the split
+//       tables take the place of split K / V and raw before the loop) | relh_s [64][h] | relw_s [64][w]
+struct SplitAttnArgs {
+  const float* qkv;   // [B*N, 3C]
+  const float* th;    // [2h-1, 64]
+  const float* tw;    // [2w-1, 64]
+  float* out;         // [B*N, C]
+  int h, w, N, heads;
+};
+
+// Split 8 fp32 values into the three bf16 terms and store them as 16-byte chunk `ch` of row `row` of three swizzled
+// tiles `tstride` bytes apart (term order h, m, l).
+__device__ __forceinline__ void store_split8(uint32_t s, uint32_t tstride, int row, int ch, const float (&x)[8]) {
+  uint32_t t[3][4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    __nv_bfloat16 a[3], b[3];
+    split3(x[2 * j], a);
+    split3(x[2 * j + 1], b);
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+      t[k][j] = static_cast<uint32_t>(__bfloat16_as_ushort(a[k])) |
+                static_cast<uint32_t>(__bfloat16_as_ushort(b[k])) << 16;
+  }
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(s + k * tstride + sw128(row, ch)), "r"(t[k][0]),
+                 "r"(t[k][1]), "r"(t[k][2]), "r"(t[k][3]) : "memory");
+}
+// 8 fp32 from global (16-byte aligned), zeros when !valid
+__device__ __forceinline__ void load8(const float* g, bool valid, float (&x)[8]) {
+  float4 u = make_float4(0.f, 0.f, 0.f, 0.f), v = u;
+  if (valid) {
+    u = reinterpret_cast<const float4*>(g)[0];
+    v = reinterpret_cast<const float4*>(g)[1];
+  }
+  x[0] = u.x; x[1] = u.y; x[2] = u.z; x[3] = u.w;
+  x[4] = v.x; x[5] = v.y; x[6] = v.z; x[7] = v.w;
+}
+
+__global__ void __launch_bounds__(AT_THREADS)
+attn_fwd_split3_kernel(const SplitAttnArgs a) {
+  extern __shared__ uint8_t smem_raw[];
+  uint32_t sQ;
+  uint8_t* sm = aligned_smem(smem_raw, sQ);
+  const int h = a.h, w = a.w, N = a.N, C = a.heads * 64;
+  const uint32_t sKV = sQ + 3 * AT_TILE, sRaw = sKV + 6 * AT_TILE;
+  const size_t tb = table_bytes(h, w), area = 3 * tb > 10 * AT_TILE ? 3 * tb : 10 * AT_TILE;
+  float* relh_s = reinterpret_cast<float*>(sm + 3 * AT_TILE + area);
+  float* relw_s = relh_s + AT_BM * h;
+  const int q0 = blockIdx.x * AT_BM, head = blockIdx.y, b = blockIdx.z;
+  const float* base = a.qkv + static_cast<size_t>(b) * N * 3 * C;
+  pdl_launch_dependents();
+  pdl_wait();
+
+  // split Q tile and split tables (in the K / V area), then the bias rows
+#pragma unroll
+  for (int it = 0; it < (AT_BM * 8) / AT_THREADS; ++it) {
+    const int idx = it * AT_THREADS + threadIdx.x, row = idx >> 3, ch = idx & 7;
+    float x[8];
+    load8(base + static_cast<size_t>(q0 + row) * 3 * C + head * 64 + ch * 8, q0 + row < N, x);
+    store_split8(sQ, AT_TILE, row, ch, x);
+  }
+  {
+    const int Lh = 2 * h - 1, Lw = 2 * w - 1, hp = tab_h_rows(h), rows = static_cast<int>(tb / 128);
+    for (int idx = threadIdx.x; idx < rows * 8; idx += AT_THREADS) {
+      const int row = idx >> 3, ch = idx & 7;
+      const bool hs = row < hp;
+      const int tr = hs ? row : row - hp;
+      float x[8];
+      load8((hs ? a.th : a.tw) + static_cast<size_t>(tr) * 64 + ch * 8, tr < (hs ? Lh : Lw), x);
+      store_split8(sKV, static_cast<uint32_t>(tb), row, ch, x);
+    }
+  }
+  fence_proxy_async_smem();
+  __syncthreads();
+  bias_rows_product<true>(h, w, N, sQ, sKV, static_cast<uint32_t>(tb), q0, relh_s, relw_s);
+  __syncthreads();   // the tables are dead: split K / V and the raw tiles take their place
+
+  // raw K / V tile t: each fp32 row of 64 is read as 128 bf16-sized columns, 32 fp32 per swizzled tile
+  const int ntiles = (N + AT_BM - 1) / AT_BM;
+  const __nv_bfloat16* raw = reinterpret_cast<const __nv_bfloat16*>(base);
+  auto issue = [&](int t) {
+    if (t < ntiles) {
+#pragma unroll
+      for (int m = 0; m < 2; ++m)
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+          load_tile(sRaw + (2 * m + j) * AT_TILE, raw, 6 * C, t * AT_BM, N, 2 * ((m + 1) * C + head * 64) + 64 * j);
+    }
+    cp_async_commit();
+  };
+  issue(0);
+
+  const int lane = threadIdx.x & 31, g = lane >> 2, c2 = 2 * (lane & 3);
+  const int rl0 = (threadIdx.x >> 5) * 16 + g;
+  const int dr = AT_BM / w, dc = AT_BM - dr * w;
+  int kr[16], kc[16];
+  key_coords_init(c2, w, kr, kc);
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  float o[32], s[32], pv[32];
+  zero32(o);
+  zero32(s);
+  zero32(pv);
+
+  for (int t = 0; t < ntiles; ++t) {
+    cp_async_wait<0>();
+    __syncthreads();   // raw tile t has landed; the products of tile t - 1 are done with split K / V
+    // split: output chunk ch of a row covers fp32 columns [8 ch, 8 ch + 8): raw tile ch / 4, raw chunks 2 (ch % 4) (+1)
+#pragma unroll
+    for (int it = 0; it < (2 * AT_BM * 8) / AT_THREADS; ++it) {
+      const int idx = it * AT_THREADS + threadIdx.x, mat = idx >> 9, row = (idx >> 3) & 63, ch = idx & 7;
+      const uint32_t src = sRaw + (2 * mat + (ch >> 2)) * AT_TILE;
+      float x[8];
+      asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(x[0]), "=f"(x[1]), "=f"(x[2]), "=f"(x[3])
+                   : "r"(src + sw128(row, 2 * (ch & 3))) : "memory");
+      asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(x[4]), "=f"(x[5]), "=f"(x[6]), "=f"(x[7])
+                   : "r"(src + sw128(row, 2 * (ch & 3) + 1)) : "memory");
+      store_split8(sKV + mat * 3 * AT_TILE, AT_TILE, row, ch, x);
+    }
+    fence_proxy_async_smem();
+    __syncthreads();   // split tiles visible to wgmma; the raw tiles are free
+    issue(t + 1);
+    const uint32_t sK = sKV, sV = sKV + 3 * AT_TILE;
+    const int k0 = t * AT_BM;
+    wgmma_fence_operands(s);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 6; ++k) mma_ss(s, sQ + c_termA[k] * AT_TILE, sK + c_termB[k] * AT_TILE, k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operands(s);
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int key = k0 + nt * 8 + c2 + (e & 1), r = rl0 + 8 * (e >> 1);
+        const int j = 2 * nt + (e & 1);
+        float v = -INFINITY;
+        if (key < N) v = fmaf(s[4 * nt + e], 0.125f, relh_s[r * h + kr[j]] + relw_s[r * w + kc[j]]);
+        s[4 * nt + e] = v;
+        mx[e >> 1] = fmaxf(mx[e >> 1], v);
+      }
+    float alpha[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 1));
+      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 2));
+      const float mn = fmaxf(m[i], mx[i]);
+      alpha[i] = expf(m[i] - mn);   // m = -inf on the first tile: alpha = 0 (nothing accumulated yet)
+      m[i] = mn;
+      l[i] *= alpha[i];
+    }
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const float p = expf(s[i] - m[(i >> 1) & 1]);
+      s[i] = p;
+      l[(i >> 1) & 1] += p;
+    }
+    // P as three register fragments: h = bf16(p), m = bf16(p - h), l = bf16(p - h - m) (the differences are exact)
+    uint32_t pa[3][4][4];
+    pack_frag(s, pa[0]);
+#pragma unroll
+    for (int i = 0; i < 32; ++i) s[i] -= bf16_round(s[i]);
+    pack_frag(s, pa[1]);
+#pragma unroll
+    for (int i = 0; i < 32; ++i) s[i] -= bf16_round(s[i]);
+    pack_frag(s, pa[2]);
+    // this tile's P V starts from zero, smallest terms first, and is added to O in fp32: the small terms are never
+    // summed into the running O inside the tensor core, which does not round them like an fp32 add
+    wgmma_fence_operands(pv);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 6; ++k) mma_rs(pv, pa[c_termA[k]], sV + c_termB[k] * AT_TILE, k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operands(pv);
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = fmaf(o[i], alpha[(i >> 1) & 1], pv[i]);
+    key_coords_next(dr, dc, w, kr, kc);
+  }
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    l[i] += __shfl_xor_sync(0xffffffffu, l[i], 1);
+    l[i] += __shfl_xor_sync(0xffffffffu, l[i], 2);
+  }
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int t = q0 + rl0 + 8 * i;
+    if (t >= N) continue;
+    const float inv = 1.0f / l[i];
+    float* orow = a.out + (static_cast<size_t>(b) * N + t) * C + head * 64;
+#pragma unroll
+    for (int dt = 0; dt < 8; ++dt)
+      *reinterpret_cast<float2*>(orow + dt * 8 + c2) = make_float2(o[4 * dt + 2 * i] * inv, o[4 * dt + 2 * i + 1] * inv);
+  }
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -819,8 +1048,8 @@ static AttnArgs attn_args(const void* qkv, const void* th, const void* tw, int B
   return a;
 }
 
-static int launch_attn(void (*kernel)(AttnArgs), dim3 grid, size_t smem, cudaStream_t st, const AttnArgs& a,
-                       const char* who) {
+template <class Args>
+static int launch_attn(void (*kernel)(Args), dim3 grid, size_t smem, cudaStream_t st, const Args& a, const char* who) {
   PK_CHECK(smem <= 227 * 1024, "%s: h=%d w=%d needs %zu B of shared memory", who, a.h, a.w, smem);
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
   PK_CHECK(e == cudaSuccess, "%s: cudaFuncSetAttribute: %s", who, cudaGetErrorString(e));
@@ -860,6 +1089,21 @@ extern "C" int pk_attn_fwd_save(const void* qkv, const void* th, const void* tw,
                                 float* relw_g, int B, int heads, int h, int w, int th_pad, int tw_pad, void* stream) {
   PK_CHECK(lse && relh_g && relw_g, "pk_attn_fwd_save: null pointer");
   return attn_fwd_impl(qkv, th, tw, out, lse, relh_g, relw_g, B, heads, h, w, th_pad, tw_pad, stream);
+}
+
+// fp32-accurate forward: qkv fp32 [B*N, 3C] (the qkv GEMM's layout), th / tw the fp32 tables [2h-1, 64] /
+// [2w-1, 64], out fp32 [B*N, C] (heads merged, like pk_attn_fwd)
+extern "C" int pk_attn_fwd_split3(const float* qkv, const float* th, const float* tw, float* out, int B, int heads,
+                                  int h, int w, void* stream) {
+  PK_CHECK(qkv && th && tw && out, "pk_attn_fwd_split3: null pointer");
+  PK_CHECK(B > 0 && heads > 0 && h > 0 && w > 0 && h <= 112 && w <= 56, "pk_attn_fwd_split3: bad shape h=%d w=%d", h,
+           w);
+  SplitAttnArgs a{qkv, th, tw, out, h, w, h * w, heads};
+  const size_t tb = table_bytes(h, w);
+  const size_t smem = 1024 + 3 * AT_TILE + (3 * tb > 10 * AT_TILE ? 3 * tb : 10 * AT_TILE) +
+                      static_cast<size_t>(AT_BM) * (h + w) * 4;
+  const dim3 grid((a.N + AT_BM - 1) / AT_BM, heads, B);
+  return launch_attn(attn_fwd_split3_kernel, grid, smem, static_cast<cudaStream_t>(stream), a, "pk_attn_fwd_split3");
 }
 
 // qkv / dqkv: bf16 [B*N, 3C];  O, dO: bf16 [B*N, C];  lse: fp32 [B*heads, N] from pk_attn_fwd

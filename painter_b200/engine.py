@@ -172,8 +172,6 @@ class BlockFn(torch.autograd.Function):
         save_rel = False
         relh = relw = x.new_empty(0)
         if ws > 0:
-            if ens_groups > 0:
-                raise NotImplementedError("painter_b200: prompt ensemble inside a windowed block")
             u = ops.window_partition_bf16(u, Bp, h, w, ws)   # zero-padded windows [Bp*nW*ws*ws, C]
             Bw = u.shape[0] // (ws * ws)
             qkv = ops.gemm(u, wqkv, kind=EPI_BF16, bias=qkv_b)
@@ -182,7 +180,10 @@ class BlockFn(torch.autograd.Function):
             else:
                 ao, lse = ops.attn_fwd(qkv, th, tw, Bw, heads, ws, ws)
             a = ops.gemm(ao, wproj, kind=EPI_F32, bias=proj_b)
-            x1 = ops.window_unpartition(a, Bp, h, w, ws, resid=x, rowscale=drop_a)
+            if ens_groups > 0:   # the ensemble merges on the full token grid, after window_unpartition
+                x1 = ops.ensemble_resid(ops.window_unpartition(a, Bp, h, w, ws), x, ens_groups, ens_P, N, C)
+            else:
+                x1 = ops.window_unpartition(a, Bp, h, w, ws, resid=x, rowscale=drop_a)
         else:
             qkv = ops.gemm(u, wqkv, kind=EPI_BF16, bias=qkv_b)
             if save_rel:

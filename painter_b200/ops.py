@@ -126,6 +126,22 @@ def attn_fwd(qkv, th, tw, B, heads, h, w, need_lse=True, save_rel=False):
     return out, lse
 
 
+def attn_fwd_split3(qkv, th, tw, B, heads, h, w):
+    """fp32-accurate fused attention forward (split-bf16 products, accumulated in fp32).  qkv: fp32 [B*h*w, 3*heads*64];
+    th / tw: fp32 rel-pos tables [2h-1, 64] / [2w-1, 64].  Returns out fp32 [B*h*w, heads*64]."""
+    _req(qkv, torch.float32, "qkv")
+    _req(th, torch.float32, "th")
+    _req(tw, torch.float32, "tw")
+    N, C = h * w, heads * 64
+    assert qkv.is_contiguous() and tuple(qkv.shape) == (B * N, 3 * C)
+    assert th.is_contiguous() and tw.is_contiguous()
+    assert tuple(th.shape) == (2 * h - 1, 64) and tuple(tw.shape) == (2 * w - 1, 64)
+    out = torch.empty((B * N, C), dtype=torch.float32, device=qkv.device)
+    check(lib().pk_attn_fwd_split3(_ptr(qkv), _ptr(th), _ptr(tw), _ptr(out), B, heads, h, w, _stream()),
+          "pk_attn_fwd_split3")
+    return out
+
+
 def attn_bwd(qkv, out, dout, lse, th, tw, B, heads, h, w, L_h=None, L_w=None, dT_out=None, rel=None):
     """Fused attention backward.  Returns (dqkv bf16 [B*N, 3C], dTh fp32 [2h-1, 64], dTw fp32 [2w-1, 64]).
     rel: the (relh, relw) buffers of `attn_fwd(..., save_rel=True)` on the same operands (the dQ kernel then loads its
