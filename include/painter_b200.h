@@ -231,7 +231,9 @@ int pk_set_pdl(int on);
 /* ------------------------------------------------------------------------------------------------
  * Inference pre/post-processing on the device (SURVEY §8 f.2).  Replaces the numpy / torch-CPU arithmetic around the
  * forward in SegGPT/SegGPT_inference/seggpt_engine.py:26-53 (run_one_image), :56-103 (inference_image), :106-181
- * (inference_video) and Painter/eval/ade20k_semantic/painter_inference_segm.py:67-93 (run_one_image).
+ * (inference_video) and the run_one_image of the Painter eval scripts Painter/eval/ade20k_semantic/
+ * painter_inference_segm.py:67-93, coco_panoptic/painter_inference_pano_{semseg,inst}.py, mmpose_custom/
+ * painter_inference_pose.py, nyuv2_depth/painter_inference_depth.py and {sidd,lol,derain}/painter_inference_*.py.
  * dtype codes of image sources: 0 = uint8 (divided by 255.), 1 = fp32 in [0,1], 2 = fp64 in [0,1].
  *  pk_stitch_normalize  canvas[p,c,y,x] fp32 NCHW [P,3,2S,S] = ((top|bottom)[p][y%S,x,c] - mean_c) / std_c in fp64
  *                       (:75-91 stitch + ImageNet normalisation, :29-34 nhwc->nchw .float()); host arrays of P device
@@ -240,7 +242,18 @@ int pk_set_pdl(int on);
  *  pk_seg_postprocess   out fp64 [h*p/2, w*p, 3] = clip((unpatchify(patch)[0, bottom half] * std + mean) * 255, 0, 255)
  *                       (:48-52); bin (nullable) fp32 [h*p/2, w*p] = mean_c(out) > 128 (:164-169, video cache)
  *  pk_nearest_blend     dst uint8 [OH,OW,3] = uint8(image * (0.6 * nearest(seg) / 255 + 0.4)) (:93-102)
- *  pk_bilinear_u8       dst uint8 [OH,OW,3] = uint8(int(bilinear(seg))) (painter_inference_segm.py:89-92)        */
+ *  pk_bilinear_u8       dst uint8 [OH,OW,3] = uint8(int(bilinear(seg))) (painter_inference_segm.py:89-92)
+ *  pk_denorm_bottom     out fp64 [h*p/2, w*p, 3] = finish(unpatchify(patch)[0, bottom half] * std + mean); finish:
+ *                       0 = clip(x * 255, 0, 255) (pk_seg_postprocess without bin), 1 = clip(x * 10000, 0, 10000)
+ *                       (painter_inference_depth.py), 2 = x (painter_inference_{sidd,lol,derain}.py)
+ *  pk_bicubic_f64       dst fp64 [OH,OW,3] = F.interpolate(src, mode='bicubic') as torch-CPU computes it on the
+ *                       float64 channels-last tensor, unclipped ({sidd,lol,derain} run_one_image, the returned array)
+ *  pk_depth_finish      dst int32 [OH,OW] = int(bilinear(src).mean(-1)) (painter_inference_depth.py run_one_image);
+ *                       cl_form selects torch-CPU's channels-last summation order (it takes that kernel on one
+ *                       thread or when OH + OW <= 128), else its generic one
+ *  pk_nearest_u8        dst uint8 [OH,OW,3] = uint8(int(nearest(src))) (painter_inference_pano_inst.py,
+ *                       painter_inference_pose.py run_one_image); cl_form selects torch-CPU's channels-last source
+ *                       index (it takes that kernel when OH + OW <= 128), else its generic one                      */
 int pk_stitch_normalize(const void* const* top, const int* top_dtype, const void* const* bottom,
                         const int* bottom_dtype, float* out, int P, int S, void* stream);
 int pk_nhwc_to_nchw_f32(const void* in, int in_is_f64, float* out, int n, int H, int W, void* stream);
@@ -248,6 +261,10 @@ int pk_seg_postprocess(const float* patch, double* out, float* bin_or_null, int 
 int pk_nearest_blend(const double* seg, int SH, int SW, const uint8_t* image, uint8_t* dst, int OH, int OW,
                      void* stream);
 int pk_bilinear_u8(const double* seg, int SH, int SW, uint8_t* dst, int OH, int OW, void* stream);
+int pk_denorm_bottom(const float* patch, double* out, int h, int w, int p, int finish, void* stream);
+int pk_bicubic_f64(const double* src, int SH, int SW, double* dst, int OH, int OW, void* stream);
+int pk_depth_finish(const double* src, int SH, int SW, int32_t* dst, int OH, int OW, int cl_form, void* stream);
+int pk_nearest_u8(const double* src, int SH, int SW, uint8_t* dst, int OH, int OW, int cl_form, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * fp32-accurate forward mode (north star: within 1e-5 of the reference's fp32 forward, the way

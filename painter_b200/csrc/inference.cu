@@ -1,12 +1,15 @@
 // painter_b200 — device-side pre/post-processing of the inference wrappers (SURVEY §8 f.2): everything the reference
 // does in numpy / PIL-free torch around the forward of seggpt_engine.inference_image / inference_video
-// (SegGPT/SegGPT_inference/seggpt_engine.py:56-181) and painter_inference_segm.run_one_image
-// (Painter/eval/ade20k_semantic/painter_inference_segm.py:67-93), so that a frame costs one small H2D copy, the
-// forward, and one D2H copy of the finished uint8 image.
+// (SegGPT/SegGPT_inference/seggpt_engine.py:56-181) and of the Painter eval scripts' run_one_image
+// (Painter/eval/{ade20k_semantic, coco_panoptic, mmpose_custom, nyuv2_depth, sidd, lol, derain}/painter_inference_*.py),
+// so that a frame costs one small H2D copy, the forward, and one D2H copy of the finished image (uint8 / int32 PNG,
+// or the float64 restoration result).
 //
-// The reference does this arithmetic in float64 (numpy broadcasting of the float64 mean/std arrays); the kernels
-// below keep float64 wherever the reference result is consumed as float64, so results are bit-comparable.
-// All kernels are HBM-bound streaming passes over <= a few MB.
+// The reference does this arithmetic in float64 (numpy broadcasting of the float64 mean/std arrays, torch-CPU
+// F.interpolate on the float64 tensor); the kernels below keep float64 wherever the reference result is consumed as
+// float64, so results are bit-comparable.  Where torch-CPU's compiled kernels contract a multiply and an add into one
+// fused multiply-add the kernels say so with __fma_rn; everything else is an explicitly rounded __dmul_rn / __dadd_rn.
+// All kernels are HBM-bound streaming passes over <= a few MB on the caller's stream (graph-capturable).
 #include "common.cuh"
 #include "host_common.h"
 #include "../../include/painter_b200.h"
@@ -67,10 +70,17 @@ nhwc_to_nchw_f32_kernel(const void* __restrict__ in, int in_is_f64, float* __res
   }
 }
 
-// out[y, x, c] (fp64 [H/2, W, 3]) = clip((pred_pixel(sample 0, y + H/2, x, c) * std[c] + mean[c]) * 255, 0, 255)
+// How the de-normalised bottom half is finished (the eval scripts differ only here before the resize):
+//   kClip255   clip(x * 255, 0, 255)      ade20k_semantic, coco_panoptic, mmpose_custom, seggpt_engine.py:48-52
+//   kClip10000 clip(x * 10000, 0, 10000)  nyuv2_depth/painter_inference_depth.py
+//   kPlain     x                          sidd / lol / derain (no clip)
+enum DenormFinish { kClip255 = 0, kClip10000 = 1, kPlain = 2 };
+
+// out[y, x, c] (fp64 [H/2, W, 3]) = finish(pred_pixel(sample 0, y + H/2, x, c) * std[c] + mean[c])
 // patch: patchified prediction [B, h*w, p*p*3] fp32 (inner order (pr, pc, c), models_painter.py:355-368);
-// = unpatchify -> 'nchw->nhwc' -> bottom half -> de-normalise (seggpt_engine.py:48-52).  Optionally also writes
-// bin[y, x] = (mean_c(out) > 128) (the video path's next-frame target, seggpt_engine.py:164-169).
+// = unpatchify -> 'nchw->nhwc' -> bottom half -> de-normalise (seggpt_engine.py:48-52).  Optionally (kClip255 only)
+// also writes bin[y, x] = (mean_c(out) > 128) (the video path's next-frame target, seggpt_engine.py:164-169).
+template <int kFinish>
 __global__ void __launch_bounds__(256)
 seg_postprocess_kernel(const float* __restrict__ patch, double* __restrict__ out, float* __restrict__ bin, int h,
                        int w, int p) {
@@ -85,12 +95,18 @@ seg_postprocess_kernel(const float* __restrict__ patch, double* __restrict__ out
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       // explicit IEEE mul / add: numpy rounds the product before the addition (no fused multiply-add)
-      double v = __dmul_rn(__dadd_rn(__dmul_rn(static_cast<double>(src[c]), c_std[c]), c_mean[c]), 255.0);
-      v = v < 0.0 ? 0.0 : (v > 255.0 ? 255.0 : v);
+      double v = __dadd_rn(__dmul_rn(static_cast<double>(src[c]), c_std[c]), c_mean[c]);
+      if (kFinish == kClip255) {
+        v = __dmul_rn(v, 255.0);
+        v = v < 0.0 ? 0.0 : (v > 255.0 ? 255.0 : v);
+      } else if (kFinish == kClip10000) {
+        v = __dmul_rn(v, 10000.0);
+        v = v < 0.0 ? 0.0 : (v > 10000.0 ? 10000.0 : v);
+      }
       out[i * 3 + c] = v;
       s += v;
     }
-    if (bin) bin[i] = (s / 3.0 > 128.0) ? 1.f : 0.f;
+    if (kFinish == kClip255 && bin) bin[i] = (s / 3.0 > 128.0) ? 1.f : 0.f;
   }
 }
 
@@ -120,6 +136,32 @@ nearest_blend_kernel(const double* __restrict__ seg, int SH, int SW, const uint8
   }
 }
 
+// One axis of ATen's linear interpolation (align_corners=False, scale = in / out from the sizes):
+// compute_source_index_and_lambda.  src = scale * (dst + 0.5) - 0.5 (one fused multiply-add in torch-CPU's build),
+// clamped at 0; i1 = i0 + 1 inside the image; l1 = src - i0, l0 = 1 - l1.  An unchanged size copies (l1 = 0).
+struct LinearTap {
+  int i0, i1;
+  double l0, l1;
+};
+__device__ __forceinline__ LinearTap linear_tap(int dst, int in_size, int out_size, double scale) {
+  LinearTap t;
+  if (in_size == out_size) {
+    t.i0 = t.i1 = dst;
+    t.l0 = 1.0;
+    t.l1 = 0.0;
+    return t;
+  }
+  double f = __fma_rn(scale, static_cast<double>(dst) + 0.5, -0.5);
+  if (f < 0.0) f = 0.0;
+  t.i0 = static_cast<int>(f);
+  if (t.i0 > in_size - 1) t.i0 = in_size - 1;
+  t.i1 = t.i0 + (t.i0 < in_size - 1 ? 1 : 0);
+  t.l1 = __dadd_rn(f, -static_cast<double>(t.i0));
+  t.l1 = t.l1 < 0.0 ? 0.0 : (t.l1 > 1.0 ? 1.0 : t.l1);
+  t.l0 = __dadd_rn(1.0, -t.l1);
+  return t;
+}
+
 // dst[y, x, c] (uint8 [OH, OW, 3]) = uint8(int(bilinear(seg)[y, x, c]))   (painter_inference_segm.py:89-92:
 // F.interpolate(mode='bilinear', align_corners=False) on the float64 tensor, .int(), astype(uint8))
 __global__ void __launch_bounds__(256)
@@ -131,15 +173,145 @@ bilinear_u8_kernel(const double* __restrict__ seg, int SH, int SW, uint8_t* __re
     const int c = static_cast<int>(i % 3);
     const size_t r = i / 3;
     const int x = static_cast<int>(r % OW), y = static_cast<int>(r / OW);
-    double fy = sch * (y + 0.5) - 0.5, fx = scw * (x + 0.5) - 0.5;
-    if (fy < 0.0) fy = 0.0;
-    if (fx < 0.0) fx = 0.0;
-    const int y0 = static_cast<int>(fy), x0 = static_cast<int>(fx);
-    const int y1 = y0 + (y0 < SH - 1 ? 1 : 0), x1 = x0 + (x0 < SW - 1 ? 1 : 0);
-    const double ly = fy - y0, lx = fx - x0, hy = 1.0 - ly, hx = 1.0 - lx;
+    const LinearTap ty = linear_tap(y, SH, OH, sch), tx = linear_tap(x, SW, OW, scw);
     auto at = [&](int yy, int xx) { return seg[(static_cast<size_t>(yy) * SW + xx) * 3 + c]; };
-    const double v = hy * (hx * at(y0, x0) + lx * at(y0, x1)) + ly * (hx * at(y1, x0) + lx * at(y1, x1));
+    const double v = ty.l0 * (tx.l0 * at(ty.i0, tx.i0) + tx.l1 * at(ty.i0, tx.i1)) +
+                     ty.l1 * (tx.l0 * at(ty.i1, tx.i0) + tx.l1 * at(ty.i1, tx.i1));
     dst[i] = static_cast<uint8_t>(static_cast<int>(v));
+  }
+}
+
+// dst[y, x] (int32 [OH, OW]) = int(mean_c(bilinear(src)[y, x, c]))   (nyuv2_depth/painter_inference_depth.py:
+// F.interpolate(mode='bilinear') on the float64 tensor, .mean(-1), .int()).  torch-CPU evaluates the 2 x 2 sum in one
+// of two forms, both reproduced here with the fused multiply-adds of its build:
+//   cl_form = 0 (its generic kernel)        (v00 l0x + v01 l1x) l0y + (v10 l0x + v11 l1x) l1y
+//   cl_form = 1 (its channels-last kernel)  v00 (l0y l0x) + v01 (l0y l1x) + v10 (l1y l0x) + v11 (l1y l1x), left to right
+// The mean is torch's sum over the 3 channels in order, then / 3.
+__global__ void __launch_bounds__(256)
+depth_finish_kernel(const double* __restrict__ src, int SH, int SW, int32_t* __restrict__ dst, int OH, int OW,
+                    int cl_form) {
+  const size_t total = static_cast<size_t>(OH) * OW;
+  const double sch = static_cast<double>(SH) / OH, scw = static_cast<double>(SW) / OW;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const int x = static_cast<int>(i % OW), y = static_cast<int>(i / OW);
+    const LinearTap ty = linear_tap(y, SH, OH, sch), tx = linear_tap(x, SW, OW, scw);
+    const double* r0 = src + static_cast<size_t>(ty.i0) * SW * 3;
+    const double* r1 = src + static_cast<size_t>(ty.i1) * SW * 3;
+    const double w00 = __dmul_rn(ty.l0, tx.l0), w01 = __dmul_rn(ty.l0, tx.l1);
+    const double w10 = __dmul_rn(ty.l1, tx.l0), w11 = __dmul_rn(ty.l1, tx.l1);
+    double s = 0.0;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const double v00 = r0[tx.i0 * 3 + c], v01 = r0[tx.i1 * 3 + c];
+      const double v10 = r1[tx.i0 * 3 + c], v11 = r1[tx.i1 * 3 + c];
+      double v;
+      if (cl_form) {
+        v = __fma_rn(v11, w11, __fma_rn(v10, w10, __fma_rn(v00, w00, __dmul_rn(v01, w01))));
+      } else {
+        const double t0 = __fma_rn(v00, tx.l0, __dmul_rn(v01, tx.l1));
+        const double t1 = __fma_rn(v10, tx.l0, __dmul_rn(v11, tx.l1));
+        v = __fma_rn(t0, ty.l0, __dmul_rn(t1, ty.l1));
+      }
+      s = c == 0 ? v : __dadd_rn(s, v);
+    }
+    dst[i] = static_cast<int32_t>(__ddiv_rn(s, 3.0));   // .int(): truncation (values are within [0, 10000])
+  }
+}
+
+// ATen's nearest source index in its generic kernel (HelperInterpNearest): scale = double(in) / out, then
+// floorf(scale * dst) of the product rounded to float.  Its channels-last kernel uses nearest_idx above instead.
+__device__ __forceinline__ int nearest_idx_generic(int dst, int in_size, double scale) {
+  const int s = static_cast<int>(floorf(static_cast<float>(__dmul_rn(scale, static_cast<double>(dst)))));
+  return s < in_size - 1 ? s : in_size - 1;
+}
+
+// dst[y, x, c] (uint8 [OH, OW, 3]) = uint8(int(nearest(src)[y, x, c]))   (coco_panoptic/painter_inference_pano_inst.py,
+// mmpose_custom/painter_inference_pose.py: F.interpolate(mode='nearest') on the float64 tensor, .int(), astype(uint8)).
+// cl_form = 1: torch-CPU's channels-last kernel (which it takes for 3 channels when OH + OW <= 128), else its generic
+// kernel; the two compute the source index differently.
+__global__ void __launch_bounds__(256)
+nearest_u8_kernel(const double* __restrict__ src, int SH, int SW, uint8_t* __restrict__ dst, int OH, int OW,
+                  int cl_form) {
+  const size_t total = static_cast<size_t>(OH) * OW * 3;
+  const double sch = static_cast<double>(SH) / OH, scw = static_cast<double>(SW) / OW;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const int c = static_cast<int>(i % 3);
+    const size_t r = i / 3;
+    const int x = static_cast<int>(r % OW), y = static_cast<int>(r / OW);
+    const int sy = cl_form ? nearest_idx(y, SH, OH) : nearest_idx_generic(y, SH, sch);
+    const int sx = cl_form ? nearest_idx(x, SW, OW) : nearest_idx_generic(x, SW, scw);
+    dst[i] = static_cast<uint8_t>(static_cast<int>(src[(static_cast<size_t>(sy) * SW + sx) * 3 + c]));
+  }
+}
+
+// ATen's cubic convolution weights (get_cubic_upsample_coefficients, A = -0.75) of the 4 taps around a source
+// position with fractional part t, with the fused multiply-adds of torch-CPU's build:
+//   w(x) = ((A + 2) x - (A + 3)) x x + 1      for the two inner taps (x = t, 1 - t)
+//   w(x) = ((A x - 5A) x + 8A) x - 4A         for the two outer taps (x = t + 1, (1 - t) + 1)
+__device__ __forceinline__ double cubic_inner(double x) {
+  const double A = -0.75;
+  return __dadd_rn(__dmul_rn(__dmul_rn(__fma_rn(A + 2.0, x, -(A + 3.0)), x), x), 1.0);
+}
+__device__ __forceinline__ double cubic_outer(double x) {
+  const double A = -0.75;
+  return __dadd_rn(__dmul_rn(__fma_rn(__fma_rn(A, x, -5.0 * A), x, 8.0 * A), x), -4.0 * A);
+}
+// One axis of ATen's bicubic (align_corners=False, scale = in / out): src = scale * (dst + 0.5) - 0.5 (not clamped),
+// i = min(floorf(src), in - 1) (floorf of the value rounded to float, as ATen does), t = clamp(src - i, 0, 1); taps
+// i - 1 .. i + 2 clamped to the border.
+struct CubicTaps {
+  int idx[4];
+  double w[4];
+};
+__device__ __forceinline__ CubicTaps cubic_taps(int dst, int in_size, double scale) {
+  CubicTaps k;
+  const double f = __fma_rn(scale, static_cast<double>(dst) + 0.5, -0.5);
+  int i = static_cast<int>(floorf(static_cast<float>(f)));
+  if (i > in_size - 1) i = in_size - 1;
+  double t = __dadd_rn(f, -static_cast<double>(i));
+  t = t < 0.0 ? 0.0 : (t > 1.0 ? 1.0 : t);
+  const double u = __dadd_rn(1.0, -t);
+  k.w[0] = cubic_outer(__dadd_rn(t, 1.0));
+  k.w[1] = cubic_inner(t);
+  k.w[2] = cubic_inner(u);
+  k.w[3] = cubic_outer(__dadd_rn(u, 1.0));
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const int v = i - 1 + j;
+    k.idx[j] = v < 0 ? 0 : (v > in_size - 1 ? in_size - 1 : v);
+  }
+  return k;
+}
+// ATen's 4-tap weighted sum: fma(v3, w3, fma(v2, w2, fma(v0, w0, v1 w1)))
+__device__ __forceinline__ double cubic_sum(const double v[4], const double w[4]) {
+  return __fma_rn(v[3], w[3], __fma_rn(v[2], w[2], __fma_rn(v[0], w[0], __dmul_rn(v[1], w[1]))));
+}
+
+// dst[y, x, c] (fp64 [OH, OW, 3]) = bicubic(src)[y, x, c]   (sidd / lol / derain painter_inference_*.py:
+// F.interpolate(mode='bicubic', align_corners=False) on the float64 tensor, no clipping).  As in ATen, each of the 4
+// source rows is first summed along x, then the 4 row sums along y.
+__global__ void __launch_bounds__(256)
+bicubic_f64_kernel(const double* __restrict__ src, int SH, int SW, double* __restrict__ dst, int OH, int OW) {
+  const size_t total = static_cast<size_t>(OH) * OW * 3;
+  const double sch = static_cast<double>(SH) / OH, scw = static_cast<double>(SW) / OW;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const int c = static_cast<int>(i % 3);
+    const size_t r = i / 3;
+    const int x = static_cast<int>(r % OW), y = static_cast<int>(r / OW);
+    const CubicTaps ky = cubic_taps(y, SH, sch), kx = cubic_taps(x, SW, scw);
+    double rows[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const double* row = src + static_cast<size_t>(ky.idx[j]) * SW * 3 + c;
+      double v[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) v[k] = row[kx.idx[k] * 3];
+      rows[j] = cubic_sum(v, kx.w);
+    }
+    dst[i] = cubic_sum(rows, ky.w);
   }
 }
 
@@ -185,9 +357,24 @@ extern "C" int pk_seg_postprocess(const float* patch, double* out, float* bin_or
                                   void* stream) {
   PK_CHECK(patch && out && h > 0 && w > 0 && p > 0 && h % 2 == 0, "pk_seg_postprocess: bad arguments");
   const size_t total = static_cast<size_t>(h) * p / 2 * w * p;
-  seg_postprocess_kernel<<<stream_grid(total), 256, 0, static_cast<cudaStream_t>(stream)>>>(patch, out, bin_or_null, h,
-                                                                                            w, p);
+  seg_postprocess_kernel<kClip255><<<stream_grid(total), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      patch, out, bin_or_null, h, w, p);
   PK_LAUNCH_CHECK("pk_seg_postprocess");
+  return 0;
+}
+
+extern "C" int pk_denorm_bottom(const float* patch, double* out, int h, int w, int p, int finish, void* stream) {
+  PK_CHECK(patch && out && h > 0 && w > 0 && p > 0 && h % 2 == 0 && finish >= kClip255 && finish <= kPlain,
+           "pk_denorm_bottom: bad arguments");
+  const size_t total = static_cast<size_t>(h) * p / 2 * w * p;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (finish == kClip255)
+    seg_postprocess_kernel<kClip255><<<stream_grid(total), 256, 0, st>>>(patch, out, nullptr, h, w, p);
+  else if (finish == kClip10000)
+    seg_postprocess_kernel<kClip10000><<<stream_grid(total), 256, 0, st>>>(patch, out, nullptr, h, w, p);
+  else
+    seg_postprocess_kernel<kPlain><<<stream_grid(total), 256, 0, st>>>(patch, out, nullptr, h, w, p);
+  PK_LAUNCH_CHECK("pk_denorm_bottom");
   return 0;
 }
 
@@ -205,5 +392,31 @@ extern "C" int pk_bilinear_u8(const double* seg, int SH, int SW, uint8_t* dst, i
   bilinear_u8_kernel<<<stream_grid(static_cast<size_t>(OH) * OW * 3), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       seg, SH, SW, dst, OH, OW);
   PK_LAUNCH_CHECK("pk_bilinear_u8");
+  return 0;
+}
+
+extern "C" int pk_bicubic_f64(const double* src, int SH, int SW, double* dst, int OH, int OW, void* stream) {
+  PK_CHECK(src && dst && SH > 0 && SW > 0 && OH > 0 && OW > 0, "pk_bicubic_f64: bad arguments");
+  bicubic_f64_kernel<<<stream_grid(static_cast<size_t>(OH) * OW * 3), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      src, SH, SW, dst, OH, OW);
+  PK_LAUNCH_CHECK("pk_bicubic_f64");
+  return 0;
+}
+
+extern "C" int pk_depth_finish(const double* src, int SH, int SW, int32_t* dst, int OH, int OW, int cl_form,
+                               void* stream) {
+  PK_CHECK(src && dst && SH > 0 && SW > 0 && OH > 0 && OW > 0, "pk_depth_finish: bad arguments");
+  depth_finish_kernel<<<stream_grid(static_cast<size_t>(OH) * OW), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      src, SH, SW, dst, OH, OW, cl_form != 0);
+  PK_LAUNCH_CHECK("pk_depth_finish");
+  return 0;
+}
+
+extern "C" int pk_nearest_u8(const double* src, int SH, int SW, uint8_t* dst, int OH, int OW, int cl_form,
+                             void* stream) {
+  PK_CHECK(src && dst && SH > 0 && SW > 0 && OH > 0 && OW > 0, "pk_nearest_u8: bad arguments");
+  nearest_u8_kernel<<<stream_grid(static_cast<size_t>(OH) * OW * 3), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      src, SH, SW, dst, OH, OW, cl_form != 0);
+  PK_LAUNCH_CHECK("pk_nearest_u8");
   return 0;
 }

@@ -1,7 +1,21 @@
-"""GPU-side mirror of the Painter task-inference `run_one_image` functions (SURVEY §8 f.2), e.g.
-Painter/eval/ade20k_semantic/painter_inference_segm.py:67-93: same arguments, same PNG on disk, with the
-nhwc->nchw conversion, the forward (CUDA-graph replay), unpatchify + bottom half + de-normalisation + clip and the
-bilinear resize to the source size on the GPU; only the final uint8 image crosses back to the host."""
+"""GPU-side mirror of the Painter task-inference `run_one_image` functions (SURVEY §8 f.2): same arguments, same file
+on disk (or the same returned array), with the nhwc->nchw conversion, the forward (CUDA-graph replay), unpatchify +
+bottom half + de-normalisation and the resize to the source size on the GPU; only the finished image crosses back to
+the host.
+
+    run_one_image          Painter/eval/ade20k_semantic/painter_inference_segm.py:67-93,
+                           coco_panoptic/painter_inference_pano_semseg.py          clip(x*255), bilinear, uint8 PNG
+    run_one_image_nearest  coco_panoptic/painter_inference_pano_inst.py,
+                           mmpose_custom/painter_inference_pose.py                 clip(x*255), nearest, uint8 PNG
+    run_one_image_depth    nyuv2_depth/painter_inference_depth.py                  clip(x*10000), bilinear, channel
+                                                                                   mean, int32 PNG
+    run_one_image_restore  sidd/painter_inference_sidd.py, lol/painter_inference_lol.py,
+                           derain/painter_inference_derain.py                      x, bicubic, returns float64 array
+
+The eval scripts call the model without torch.no_grad(), so a module in precision "auto" runs its bf16 training
+arithmetic there; these mirrors run under no_grad, which selects the fp32-accurate forward (and keeps no autograd
+state), as the ADE20k mirror always has.
+"""
 import ctypes
 
 import numpy as np
@@ -9,6 +23,9 @@ import torch
 
 from ._lib import check, lib
 from .seggpt_engine import _graphed, _stream, seg_postprocess
+
+# pk_denorm_bottom finish codes
+CLIP255, CLIP10000, PLAIN = 0, 1, 2
 
 
 def bilinear_u8(seg, OH, OW):
@@ -19,11 +36,50 @@ def bilinear_u8(seg, OH, OW):
     return dst
 
 
-@torch.no_grad()
-def run_one_image(img, tgt, size, model, out_path, device):
-    """img, tgt: numpy [2*S, S, 3] ImageNet-normalised canvases; size = (width, height) of the source image; model: the
-    painter_b200 Painter module or a DistributedDataParallel wrapper of it (the script passes `model.module` users)."""
-    from PIL import Image
+def denorm_bottom(patch, h, w, p, finish):
+    """patchified prediction [B, h*w, p*p*3] fp32 -> fp64 [h*p/2, w*p, 3]: bottom half of sample 0, de-normalised,
+    then ×255 clipped (CLIP255), ×10000 clipped (CLIP10000) or left as is (PLAIN)."""
+    assert patch.dtype == torch.float32 and patch.is_contiguous()
+    out = torch.empty((h * p // 2, w * p, 3), dtype=torch.float64, device=patch.device)
+    check(lib().pk_denorm_bottom(ctypes.c_void_p(patch.data_ptr()), ctypes.c_void_p(out.data_ptr()), h, w, p, finish,
+                                 _stream()), "pk_denorm_bottom")
+    return out
+
+
+def nearest_u8(src, OH, OW):
+    """src fp64 [SH, SW, 3] -> uint8 [OH, OW, 3] = uint8(int(F.interpolate(src, mode='nearest'))).  torch-CPU
+    computes the source index in float from a float scale in its channels-last kernel (3 channels: OH + OW <= 128) and
+    from a double scale in its generic one; the same index is used here."""
+    dst = torch.empty((OH, OW, 3), dtype=torch.uint8, device=src.device)
+    cl_form = int(OH + OW <= 128)
+    check(lib().pk_nearest_u8(ctypes.c_void_p(src.data_ptr()), src.shape[0], src.shape[1],
+                              ctypes.c_void_p(dst.data_ptr()), OH, OW, cl_form, _stream()), "pk_nearest_u8")
+    return dst
+
+
+def depth_finish(src, OH, OW):
+    """src fp64 [SH, SW, 3] -> int32 [OH, OW] = F.interpolate(src, mode='bilinear').mean(-1).int().  torch-CPU sums
+    the 2 x 2 taps in its channels-last kernel's order on one thread or for OH + OW <= 128 (3 channels), else in its
+    generic kernel's order; the same order is used here, so the result is identical in either case."""
+    dst = torch.empty((OH, OW), dtype=torch.int32, device=src.device)
+    cl_form = int(torch.get_num_threads() == 1 or OH + OW <= 128)
+    check(lib().pk_depth_finish(ctypes.c_void_p(src.data_ptr()), src.shape[0], src.shape[1],
+                                ctypes.c_void_p(dst.data_ptr()), OH, OW, cl_form, _stream()), "pk_depth_finish")
+    return dst
+
+
+def bicubic_f64(src, OH, OW):
+    """src fp64 [SH, SW, 3] -> fp64 [OH, OW, 3] = F.interpolate(src, mode='bicubic') (align_corners=False, no clip)."""
+    dst = torch.empty((OH, OW, 3), dtype=torch.float64, device=src.device)
+    check(lib().pk_bicubic_f64(ctypes.c_void_p(src.data_ptr()), src.shape[0], src.shape[1],
+                               ctypes.c_void_p(dst.data_ptr()), OH, OW, _stream()), "pk_bicubic_f64")
+    return dst
+
+
+def _predict(img, tgt, model, device):
+    """The front half every eval script shares: img, tgt numpy [2*S, S, 3] ImageNet-normalised canvases ->
+    nchw fp32 on the device, the bottom-half mask, valid = 1, and one graphed forward of the module (or of the
+    `.module` of a DistributedDataParallel-style wrapper).  Returns (patchified prediction, h, w, p)."""
     device = torch.device(device)
     net = model.module if hasattr(model, "module") else model
     x = torch.as_tensor(img).unsqueeze(0).to(device, non_blocking=True)
@@ -40,7 +96,47 @@ def run_one_image(img, tgt, size, model, out_path, device):
     mask[:, n // 2:] = 1
     valid = torch.ones_like(tin)
     _, y, _ = _graphed(net)(xin, tin, mask, valid)
-    seg, _ = seg_postprocess(y, H // p, W // p, p)
+    return y, H // p, W // p, p
+
+
+@torch.no_grad()
+def run_one_image(img, tgt, size, model, out_path, device):
+    """ADE20k semantic / COCO panoptic semseg.  img, tgt: numpy [2*S, S, 3] ImageNet-normalised canvases; size =
+    (width, height) of the source image; model: the painter_b200 Painter module or a DistributedDataParallel wrapper
+    of it (the script passes `model.module` users).  Writes the uint8 PNG to out_path."""
+    from PIL import Image
+    y, h, w, p = _predict(img, tgt, model, device)
+    seg, _ = seg_postprocess(y, h, w, p)
     out = bilinear_u8(seg, size[1], size[0])
     Image.fromarray(out.cpu().numpy()).save(out_path)
     return out
+
+
+@torch.no_grad()
+def run_one_image_nearest(img, tgt, size, model, out_path, device):
+    """COCO panoptic instance / COCO pose: as run_one_image, with a nearest resize.  Writes the uint8 PNG."""
+    from PIL import Image
+    y, h, w, p = _predict(img, tgt, model, device)
+    out = nearest_u8(denorm_bottom(y, h, w, p, CLIP255), size[1], size[0])
+    Image.fromarray(out.cpu().numpy()).save(out_path)
+    return out
+
+
+@torch.no_grad()
+def run_one_image_depth(img, tgt, size, model, out_path, device):
+    """NYUv2 depth: clip(x * 10000, 0, 10000), bilinear, mean over the channels, int32.  Writes the int32 PNG (depth
+    in units of 1e-4)."""
+    from PIL import Image
+    y, h, w, p = _predict(img, tgt, model, device)
+    out = depth_finish(denorm_bottom(y, h, w, p, CLIP10000), size[1], size[0])
+    Image.fromarray(out.cpu().numpy()).save(out_path)
+    return out
+
+
+@torch.no_grad()
+def run_one_image_restore(img, tgt, size, model, out_path, device):
+    """SIDD denoising / LoL enhancement / deraining: the de-normalised prediction, bicubic-resized, unclipped.
+    Returns the float64 numpy array [height, width, 3] (the caller clips it and scores it); out_path is unused, as in
+    the reference."""
+    y, h, w, p = _predict(img, tgt, model, device)
+    return bicubic_f64(denorm_bottom(y, h, w, p, PLAIN), size[1], size[0]).cpu().numpy()

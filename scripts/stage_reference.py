@@ -7,8 +7,9 @@ executed as the live oracle / reference arm:
 
 The reference is pure Python with no setup.py, so `pip install --target oracle/_ref <reference>` has nothing to
 build (recorded in DESIGN.md); this script is the install step.  Only the files of the hot path, its two engines,
-the runtime utilities they import, the data pipeline used by the parity tests and the SegGPT example images are
-copied, byte for byte; nothing under oracle/_ref is tracked by git or imported by the product path.
+the runtime utilities they import, the task eval scripts (for their run_one_image), the data pipeline used by the
+parity tests and the SegGPT example images are copied, byte for byte; nothing under oracle/_ref is tracked by git or
+imported by the product path.
 """
 import filecmp
 import os
@@ -28,6 +29,13 @@ FILES = [
     "Painter/data/pair_transforms.py",
     "Painter/data/sampler.py",
     "Painter/eval/ade20k_semantic/painter_inference_segm.py",
+    "Painter/eval/coco_panoptic/painter_inference_pano_semseg.py",
+    "Painter/eval/coco_panoptic/painter_inference_pano_inst.py",
+    "Painter/eval/mmpose_custom/painter_inference_pose.py",
+    "Painter/eval/nyuv2_depth/painter_inference_depth.py",
+    "Painter/eval/sidd/painter_inference_sidd.py",
+    "Painter/eval/lol/painter_inference_lol.py",
+    "Painter/eval/derain/painter_inference_derain.py",
     "SegGPT/SegGPT_inference/models_seggpt.py",
     "SegGPT/SegGPT_inference/seggpt_engine.py",
     "SegGPT/SegGPT_inference/seggpt_inference.py",
