@@ -21,6 +21,8 @@
 // product, dS . E with E the tile's one-hot [key][image column | image row] matrix, and its tail runs both table
 // terms as products over the Toeplitz matrix G[q, table row] of those gradients: dQ += G [T_h; T_w] and the
 // table-gradient partials G^T Q.
+#include <type_traits>
+
 #include "common.cuh"
 #include "wgmma.cuh"
 #include "split3.cuh"
@@ -290,6 +292,27 @@ attn_fwd_kernel(const AttnArgs a) {
   float o[32], s[32];
   zero32(o);
   zero32(s);
+  const float* rh[2] = {relh_s + rl0 * h, relh_s + (rl0 + 8) * h};
+  const float* rw[2] = {relw_s + rl0 * w, relw_s + (rl0 + 8) * w};
+
+  // log2-domain scores of one key tile into s and their row maxima into mx.  The bias rows are gathered before the
+  // first use.  PARTIAL (the last tile when 64 does not divide N): keys past N score -inf by a select, and their
+  // gathers use a clamped image row.
+  auto tile_scores = [&](int k0, float (&mx)[2], auto partial) {
+    constexpr bool PARTIAL = decltype(partial)::value;
+    float bias[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const int j = 2 * (i >> 2) + (i & 1), e = (i >> 1) & 1;
+      bias[i] = rh[e][PARTIAL ? min(kr[j], h - 1) : kr[j]] + rw[e][kc[j]];
+    }
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const float v = fmaf(s[i], sc, bias[i]);
+      s[i] = PARTIAL ? (k0 + 8 * (i >> 2) + c2 + (i & 1) < N ? v : -INFINITY) : v;
+      mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
+    }
+  };
 
   for (int t = 0; t < ntiles; ++t) {
     issue(t + 1);
@@ -303,17 +326,8 @@ attn_fwd_kernel(const AttnArgs a) {
     wgmma_wait<0>();
     wgmma_fence_operands(s);
     float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-    for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int key = k0 + nt * 8 + c2 + (e & 1), r = rl0 + 8 * (e >> 1);
-        const int j = 2 * nt + (e & 1);
-        float v = -INFINITY;
-        if (key < N) v = fmaf(s[4 * nt + e], sc, relh_s[r * h + kr[j]] + relw_s[r * w + kc[j]]);
-        s[4 * nt + e] = v;
-        mx[e >> 1] = fmaxf(mx[e >> 1], v);
-      }
+    if (k0 + AT_BM <= N) tile_scores(k0, mx, std::false_type{});
+    else tile_scores(k0, mx, std::true_type{});
     float alpha[2];
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
@@ -596,7 +610,8 @@ attn_fwd_split3_kernel(const SplitAttnArgs a) {
 //   dS . E with the one-hot E[key x][column] = 1 at column (k0 + x) mod w and at column w + (k0 mod w + x) / w (image
 //   row k0 / w + that offset).  w <= 56 (attn_check) keeps w plus the tile's image rows within 64 columns; for w = 1
 //   the column part is left out and dRelw is the row sum of dRelh.  Each accumulator entry has one owner thread that
-//   adds it into drelh_s / drelw_s, tile after tile: no atomics, a fixed order, reproducible.
+//   adds it up tile after tile: no atomics, a fixed order, reproducible.  Image-column entries are summed in
+//   registers and stored to drelw_s after the loop; image-row entries are added into drelh_s.
 //   G[q, r] = dRelh[q, i_q + h - 1 - r] for the T_h rows r of the staged tables (zero outside [0, h)), likewise for
 //   T_w; the table-gradient partials of the CTA are G^T Q, ws[cta][c][table row].
 // smem: sQ | sdO | K/V ring (tables after the loop) | E | relh_s | relw_s | drelh_s | drelw_s
@@ -637,10 +652,7 @@ attn_bwd_dq_kernel(const AttnArgs a) {
       relh_s[i] = gh[i];
       drelh_s[i] = 0.f;
     }
-    for (int i = threadIdx.x; i < AT_BM * w; i += AT_THREADS) {
-      relw_s[i] = gw[i];
-      drelw_s[i] = 0.f;
-    }
+    for (int i = threadIdx.x; i < AT_BM * w; i += AT_THREADS) relw_s[i] = gw[i];
   }
 
   const int lane = threadIdx.x & 31, g = lane >> 2, c2 = 2 * (lane & 3);
@@ -651,6 +663,10 @@ attn_bwd_dq_kernel(const AttnArgs a) {
   int kr[16], kc[16];
   key_coords_init(c2, w, kr, kc);
   int kr0 = 0, kc0 = 0;              // k0 / w, k0 mod w
+  // image (row, column) of the key k0 + (threadIdx.x >> 3), the first of the four E rows this thread writes; the
+  // other three are 16 keys apart
+  const int er16 = 16 / w, ec16 = 16 - er16 * w;
+  int er = (threadIdx.x >> 3) / w, ec = (threadIdx.x >> 3) - er * w;
   float lse[2], dlt[2];
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
@@ -658,27 +674,63 @@ attn_bwd_dq_kernel(const AttnArgs a) {
     lse[i] = a.lse[bh * N + t];
     dlt[i] = a.delta[bh * N + t];
   }
+  const float* rh[2] = {relh_s + rl0 * h, relh_s + (rl0 + 8) * h};
+  const float* rw[2] = {relw_s + rl0 * w, relw_s + (rl0 + 8) * w};
   float dq[32], s[32], dp[32];
+  // dRel_w of the accumulator entries i < 28 (columns below 56 >= w): an image column has the same E column in every
+  // tile, so its sum over the key tiles stays in registers
+  float dwc[28];
+  // the image-row columns [wcols, wcols + 64 / w + 2) lie in the 8-column groups rc_lo .. rc_hi
+  const int rc_lo = wcols >> 3, rc_hi = min(7, (wcols + AT_BM / w + 1) >> 3);
   zero32(dq);
   zero32(s);
   zero32(dp);
+#pragma unroll
+  for (int i = 0; i < 28; ++i) dwc[i] = 0.f;
+
+  // dS of one tile into s.  PARTIAL (the last tile when 64 does not divide N): keys past N get dS = 0 by a select,
+  // and their bias gathers use a clamped image row
+  auto tile_ds = [&](int k0, auto partial) {
+    constexpr bool PARTIAL = decltype(partial)::value;
+    float bias[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const int j = 2 * (i >> 2) + (i & 1), e = (i >> 1) & 1;
+      bias[i] = rh[e][PARTIAL ? min(kr[j], h - 1) : kr[j]] + rw[e][kc[j]];
+    }
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const int e = (i >> 1) & 1;
+      const float p = fast_exp2(fmaf(s[i], sc, bias[i]) - lse[e]);
+      const float ds = p * (dp[i] - dlt[e]);
+      s[i] = PARTIAL ? (k0 + 8 * (i >> 2) + c2 + (i & 1) < N ? ds : 0.f) : ds;
+    }
+  };
 
   for (int t = 0; t < ntiles; ++t) {
     issue(t + 1);
     // E of this tile (the previous tile's products that read it have completed)
+    {
+      int xr = er, xc = ec;
 #pragma unroll
-    for (int it = 0; it < (AT_BM * 8) / AT_THREADS; ++it) {
-      const int x = it * (AT_THREADS / 8) + (threadIdx.x >> 3), ch = threadIdx.x & 7;
-      const int xr = kc0 + x, rofs = xr / w;
-      const int ccol = w > 1 ? xr - rofs * w : -1, rcol = wcols + rofs;
-      uint32_t v[4];
+      for (int it = 0; it < (AT_BM * 8) / AT_THREADS; ++it) {
+        const int x = it * (AT_THREADS / 8) + (threadIdx.x >> 3), ch = threadIdx.x & 7;
+        const int ccol = w > 1 ? xc : -1, rcol = wcols + xr - kr0;
+        uint32_t v[4];
 #pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        const int c = ch * 8 + 2 * u;
-        v[u] = (c == ccol || c == rcol ? 0x3F80u : 0u) | (c + 1 == ccol || c + 1 == rcol ? 0x3F800000u : 0u);
+        for (int u = 0; u < 4; ++u) {
+          const int c = ch * 8 + 2 * u;
+          v[u] = (c == ccol || c == rcol ? 0x3F80u : 0u) | (c + 1 == ccol || c + 1 == rcol ? 0x3F800000u : 0u);
+        }
+        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sE + sw128(x, ch)), "r"(v[0]), "r"(v[1]),
+                     "r"(v[2]), "r"(v[3]) : "memory");
+        xr += er16;
+        xc += ec16;
+        if (xc >= w) {
+          xc -= w;
+          ++xr;
+        }
       }
-      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sE + sw128(x, ch)), "r"(v[0]), "r"(v[1]),
-                   "r"(v[2]), "r"(v[3]) : "memory");
     }
     tiles_ready<1>();
     const uint32_t sK = ring + (t & 1) * 2 * AT_TILE, sV = sK + AT_TILE;
@@ -692,18 +744,8 @@ attn_bwd_dq_kernel(const AttnArgs a) {
     wgmma_wait<0>();
     wgmma_fence_operands(s);
     wgmma_fence_operands(dp);
-#pragma unroll
-    for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int key = k0 + nt * 8 + c2 + (e & 1), r = rl0 + 8 * (e >> 1), j = 2 * nt + (e & 1);
-        float ds = 0.f;
-        if (key < N) {
-          const float p = fast_exp2(fmaf(s[4 * nt + e], sc, relh_s[r * h + kr[j]] + relw_s[r * w + kc[j]]) - lse[e >> 1]);
-          ds = p * (dp[4 * nt + e] - dlt[e >> 1]);
-        }
-        s[4 * nt + e] = ds;
-      }
+    if (k0 + AT_BM <= N) tile_ds(k0, std::false_type{});
+    else tile_ds(k0, std::true_type{});
     uint32_t da[4][4];
     pack_frag(s, da);
     // dQ += dS . K and, into s, this tile's bias-row gradients dS . E
@@ -717,13 +759,14 @@ attn_bwd_dq_kernel(const AttnArgs a) {
     wgmma_fence_operands(dq);
     wgmma_fence_operands(s);
 #pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      const int r = rl0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + c2 + (i & 1);
-      if (col < wcols) {
-        drelw_s[r * w + col] += s[i];
-      } else {
-        const int ir = kr0 + col - wcols;
-        if (ir < h) drelh_s[r * h + ir] += s[i];
+    for (int i = 0; i < 28; ++i) dwc[i] += s[i];
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+      if (nt < rc_lo || nt > rc_hi) continue;
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const int i = 4 * nt + u, r = rl0 + 8 * (u >> 1), col = 8 * nt + c2 + (u & 1), ir = kr0 + col - wcols;
+        if (col >= wcols && ir < h) drelh_s[r * h + ir] += s[i];
       }
     }
     key_coords_next(dr, dc, w, kr, kc);
@@ -733,10 +776,21 @@ attn_bwd_dq_kernel(const AttnArgs a) {
       kc0 -= w;
       ++kr0;
     }
+    er += dr;
+    ec += dc;
+    if (ec >= w) {
+      ec -= w;
+      ++er;
+    }
     __syncthreads();   // stage t & 1 is free for tile t + 2, E for tile t + 1
   }
   load_tables(a, ring);
   cp_async_commit();
+#pragma unroll
+  for (int i = 0; i < 28; ++i) {
+    const int r = rl0 + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + c2 + (i & 1);
+    if (col < wcols) drelw_s[r * w + col] = dwc[i];
+  }
   if (w == 1 && threadIdx.x < AT_BM) {
     float acc = 0.f;
     for (int k = 0; k < h; ++k) acc += drelh_s[threadIdx.x * h + k];
@@ -766,18 +820,35 @@ attn_bwd_dq_kernel(const AttnArgs a) {
     }
     const uint64_t dt = make_wgmma_desc(ring, AT_TILE, 1024);
     wgmma_fence_operands(dq);
-    for (int kk = 0; kk < krows / 16; ++kk) {
-      uint32_t ga[4];
+    // The A fragments are built before the wgmmas that read them are issued, and those complete before the
+    // fragments are rebuilt: 64 table rows per round, then 16 at a time.
+    auto gfrag = [&](int kk, uint32_t (&ga)[4]) {
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
         const int e = u & 1, q = rl0 + 8 * e, r = 16 * kk + 8 * (u >> 1) + c2;
         ga[u] = pack_bf16x2(8.f * gval(q, iq[e], jq[e], r), 8.f * gval(q, iq[e], jq[e], r + 1));
+        asm volatile("" : "+r"(ga[u])::"memory");
       }
+    };
+    int kk = 0;
+    for (; kk + 4 <= krows / 16; kk += 4) {
+      uint32_t ga[4][4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) gfrag(kk + k, ga[k]);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_m64n64k16_rs<1>(dq, ga[k], wgmma_desc_add(dt, (kk + k) * 2048), 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+    }
+    for (; kk < krows / 16; ++kk) {
+      uint32_t ga[4];
+      gfrag(kk, ga);
       wgmma_fence();
       wgmma_m64n64k16_rs<1>(dq, ga, wgmma_desc_add(dt, kk * 2048), 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
     }
-    wgmma_commit();
-    wgmma_wait<0>();
     wgmma_fence_operands(dq);
   }
 #pragma unroll
@@ -889,12 +960,41 @@ attn_bwd_dkv_kernel(const AttnArgs a) {
     kr[i] = min(key, N - 1) / w;
     kc[i] = min(key, N - 1) - kr[i] * w;
   }
+  const bool kfull = k0 + AT_BM <= N;
   const float sc = a.scale_log2;
   float dk[32], dv[32], s[32], dp[32];
   zero32(dk);
   zero32(dv);
   zero32(s);
   zero32(dp);
+
+  // P^T into s and dS^T into dp for one query tile.  Every bias row and lse / delta value the thread needs is read
+  // before the first use.  PARTIAL (a key or query tile cut by N): P = 0 past N by a select; all reads stay inside
+  // the stage (kr / kc are clamped, queries past N read the zero-filled or zero-Q rows of the tile).
+  auto tile_p = [&](const float* relh_s, const float* relw_s, const float* lse_s, const float* dlt_s, int q0,
+                    auto partial) {
+    constexpr bool PARTIAL = decltype(partial)::value;
+    float bias[32], lq[16], dq[16];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const int q = 8 * (i >> 2) + c2 + (i & 1), e = (i >> 1) & 1;
+      bias[i] = relh_s[q * h + kr[e]] + relw_s[q * w + kc[e]];
+    }
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int q = 8 * (j >> 1) + c2 + (j & 1);
+      lq[j] = lse_s[q];
+      dq[j] = dlt_s[q];
+    }
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const int j = 2 * (i >> 2) + (i & 1), e = (i >> 1) & 1;
+      float p = fast_exp2(fmaf(s[i], sc, bias[i]) - lq[j]);
+      if (PARTIAL) p = kvalid[e] && q0 + 8 * (i >> 2) + c2 + (i & 1) < N ? p : 0.f;
+      s[i] = p;
+      dp[i] = p * (dp[i] - dq[j]);
+    }
+  };
 
   for (int t = 0; t < ntiles; ++t) {
     issue(t + STAGES - 1);
@@ -914,17 +1014,8 @@ attn_bwd_dkv_kernel(const AttnArgs a) {
     wgmma_wait<0>();
     wgmma_fence_operands(s);
     wgmma_fence_operands(dp);
-#pragma unroll
-    for (int nt = 0; nt < 8; ++nt)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int q = nt * 8 + c2 + (e & 1), i = e >> 1;
-        float p = 0.f;
-        if (kvalid[i] && q0 + q < N)
-          p = fast_exp2(fmaf(s[4 * nt + e], sc, relh_s[q * h + kr[i]] + relw_s[q * w + kc[i]]) - lse_s[q]);
-        s[4 * nt + e] = p;
-        dp[4 * nt + e] = p * (dp[4 * nt + e] - dlt_s[q]);
-      }
+    if (kfull && q0 + AT_BM <= N) tile_p(relh_s, relw_s, lse_s, dlt_s, q0, std::false_type{});
+    else tile_p(relh_s, relw_s, lse_s, dlt_s, q0, std::true_type{});
     uint32_t pa[4][4], da[4][4];
     pack_frag(s, pa);
     pack_frag(dp, da);
