@@ -21,12 +21,15 @@
 
 namespace pk {
 
-// One 64-deep K-block of one math warpgroup: acc[64 x BN] (+)= A[64 x 64] . B[64 x BN]^T (4 wgmma, K = 16 each).
+// One 64-deep K-block of one math warpgroup: acc[64 x BN] (+)= A[64 x 64] . B[64 x BN]^T (4 wgmma, K = 16 each),
+// committed as one wgmma group.  The fence and the commit sit inside the operand-layout branch, next to the wgmmas:
+// with a branch between them ptxas cannot prove the accumulators untouched and injects warpgroup.arrive (C7519).
 template <int BN, int TA, int TB>
 __device__ __forceinline__ void gemm_kblock(float (&acc)[BN / 2], uint32_t a_addr, uint32_t b_addr, bool first) {
   const uint64_t da = TA ? make_wgmma_desc(a_addr, 8192, 1024) : make_wgmma_desc(a_addr, 16, 1024);
   const uint64_t db = TB ? make_wgmma_desc(b_addr, 8192, 1024) : make_wgmma_desc(b_addr, 16, 1024);
   constexpr uint32_t a_step = TA ? 2048u : 32u, b_step = TB ? 2048u : 32u;
+  wgmma_fence();
 #pragma unroll
   for (int k = 0; k < GEMM_BK / 16; ++k) {
     const uint64_t a = wgmma_desc_add(da, k * a_step), b = wgmma_desc_add(db, k * b_step);
@@ -35,6 +38,7 @@ __device__ __forceinline__ void gemm_kblock(float (&acc)[BN / 2], uint32_t a_add
     else if constexpr (BN == 128) wgmma_m64n128k16<TA, TB>(acc, a, b, accf);
     else wgmma_m64n256k16<TA, TB>(acc, a, b, accf);
   }
+  wgmma_commit();
 }
 
 template <int KIND, int BN>
@@ -149,7 +153,6 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       mbar_wait(full_bar(s), ph);
       const uint32_t a_addr = sA + s * GEMM_A_BYTES + cw * 8192;   // 64 K-major rows / one 64-wide MN group
       const uint32_t b_addr = sB + s * B_BYTES;
-      wgmma_fence();
       if (g.transA) {
         if (g.transB) gemm_kblock<BN, 1, 1>(acc, a_addr, b_addr, kb == kb0);
         else gemm_kblock<BN, 1, 0>(acc, a_addr, b_addr, kb == kb0);
@@ -157,7 +160,6 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         if (g.transB) gemm_kblock<BN, 0, 1>(acc, a_addr, b_addr, kb == kb0);
         else gemm_kblock<BN, 0, 0>(acc, a_addr, b_addr, kb == kb0);
       }
-      wgmma_commit();
       wgmma_fence_operands(acc);
       wgmma_wait<1>();
       wgmma_fence_operands(acc);
@@ -320,14 +322,18 @@ static void plan_gemm(int M, int N, int K, int transA, int transB, const PkEpilo
   const int sms = sm_count();
   const int mt = (M + GEMM_BM - 1) / GEMM_BM;
   const bool zero_init_f32 = epi->kind == PK_EPI_F32 && epi->accumulate == 2;
-  // 128 x 128 tiles where the shape allows.  BN = 256 (128 accumulator registers per math thread) exceeds the
-  // 168-register budget of a 384-thread CTA once the epilogue's registers are live and spills; it stays reachable
-  // through pk_gemm_force_bn only.
+  // 128 x 128 tiles where the shape allows, 128 x 256 for the bf16 and GELU epilogues when that still gives every
+  // SM a tile: 8-13 % faster than BN = 128 at the ViT-L block shapes on H100 (qkv / fc1 forward, fc1 / qkv dgrad).
+  // At BN = 256 the math warpgroups hold 128 accumulator registers per thread; the kernels with the fp32, residual
+  // and GELU' epilogues spill 8-16 bytes there (ptxas -v), so those keep BN = 128.
   int BN = 64;
   if (zero_init_f32) {
     // weight-gradient GEMMs (K = tokens): take the wide tile and fill the machine with stream-K instead of
     // shrinking the tile
     if (N % 128 == 0) BN = 128;
+  } else if ((epi->kind == PK_EPI_BF16 || epi->kind == PK_EPI_GELU) && N % 256 == 0 &&
+             static_cast<long long>(mt) * (N / 256) >= sms) {
+    BN = 256;
   } else if (N % 128 == 0 && static_cast<long long>(mt) * (N / 128) >= sms / 2) {
     BN = 128;
   }

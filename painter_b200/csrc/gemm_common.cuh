@@ -132,7 +132,8 @@ static __constant__ float c_head_all[HEAD_SLOTS][392];   // only gemm.cu (EPI_HE
 
 __device__ __forceinline__ float smooth_l1(float d, int kind) {
   const float ad = fabsf(d);
-  if (kind == 0) return ad < 0.01f ? 0.5f * d * d / 0.01f : ad - 0.005f;  // smoothl1 beta=0.01
+  // smoothl1 beta=0.01 (0.5 d^2 leaves the normal range only for |d| < 2e-19, where the term is immaterial)
+  if (kind == 0) return ad < 0.01f ? div_rn_nocall(0.5f * d * d, 0.01f) : ad - 0.005f;
   if (kind == 1) return ad;                                             // l1
   if (kind == 2) return d * d;                                          // l2
   return (ad + d * d) * 0.5f;                                           // l1l2
@@ -287,7 +288,7 @@ __device__ __forceinline__ void gemm_epilogue_chunk(const PkEpilogue& e, float* 
     float4* srow = reinterpret_cast<float4*>(stg + lane * STG_LD);
     if (e.bias != nullptr) {
       const float4* b4 = reinterpret_cast<const float4*>(e.bias + col);
-      const float bsc = KIND == PK_EPI_RESID ? sc / e.alpha : 1.0f;  // rowscale also multiplies the bias
+      const float bsc = KIND == PK_EPI_RESID ? div_rn_nocall(sc, e.alpha) : 1.0f;  // rowscale also multiplies the bias
 #pragma unroll
       for (int q = 0; q < 8; ++q) {
         const float4 b = __ldg(b4 + q);
