@@ -312,6 +312,34 @@ int pk_block_masks(int* out, int B, int H, int W, int num_masking, int min_patch
 int pk_valid_maps(const float* targets, const int* rule_dev, const float* thr_dev, int* fg_zeroed, float* valid, int B,
                   int H, int W, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Training data path, the recipe's paired augmentations (Painter/main_train.py:232-262 as pairdataset.py applies them)
+ * on decoded uint8 RGB images, bit-identical to PIL / torch-CPU given the host's random draws (csrc/augment.cu).
+ * Descriptor tables are int32 device arrays, one row per job:
+ *  crop row   [src byte offset lo, hi, H, W, top, left, h, w, mode (0 bicubic, 1 nearest), flip,
+ *              tmp byte offset lo, hi]
+ *  jitter row [slot, op0..op3 (PK_JIT_*, -1 = none, in the drawn order), brightness, contrast, saturation (float
+ *              bits), hue shift (int(hue_factor * 255) mod 256)]
+ *  second-crop row [top, left, h, w, mode (0 antialiased bicubic, 1 nearest)]; a full box in nearest mode is a copy.
+ *  pk_aug_resized_crop  dst uint8 [J, S, S, 3] = resize(crop(src_j), S x S), flipped when asked (Pillow's resample).
+ *                       KP >= every bicubic job's coefficient count (2 ceil(2 max(h, w) / S) + 1 bounds it);
+ *                       max_rows >= every job's max(h, w); coef int32 [J, 2, S, KP], bounds int32 [J, 2, S, 2] and
+ *                       tmp (the first pass, max(h, w) * S * 3 bytes per bicubic job at its offset) are scratch.
+ *  pk_aug_color_jitter  ColorJitter (PIL) in place on images imgs + slot * npix * 3 (uint8 RGB), one CTA per image.
+ *  pk_aug_normalize     ToTensor + Normalize + the two-pair stitch: slot (b * P + p) * 2 + t (t = 0 image, 1 target)
+ *                       -> img / tgt fp32 [B, 3, P * S, S] rows p * S .. (p + 1) * S.
+ *  pk_aug_second_crop   row 2b + t crops img / tgt [b] fp32 [3, OH, OW] and resizes it back to OH x OW
+ *                       (torch-CPU interpolate, antialiased bicubic or nearest) into img_out / tgt_out.  wts fp32
+ *                       [2B, 2, OH, PK_AUG_AA_TAPS], bounds int32 [2B, 2, OH, 2], tmp fp32 [2B, 3, OH, OW] scratch. */
+enum { PK_AUG_CROP_FIELDS = 12, PK_AUG_JIT_FIELDS = 9, PK_AUG_SEC_FIELDS = 5, PK_AUG_AA_TAPS = 5 };
+enum { PK_JIT_BRIGHTNESS = 0, PK_JIT_CONTRAST = 1, PK_JIT_SATURATION = 2, PK_JIT_HUE = 3 };
+int pk_aug_resized_crop(const uint8_t* src, const int* jobs, int J, int S, int KP, int max_rows, int* coef, int* bounds,
+                        uint8_t* tmp, uint8_t* dst, void* stream);
+int pk_aug_color_jitter(uint8_t* imgs, const int* jobs, int n, long long npix, void* stream);
+int pk_aug_normalize(const uint8_t* slots, int B, int P, int S, float* img, float* tgt, void* stream);
+int pk_aug_second_crop(const float* img, const float* tgt, const int* jobs, int B, int OH, int OW, float* wts,
+                       int* bounds, float* tmp, float* img_out, float* tgt_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
