@@ -80,7 +80,9 @@ int pk_gemm_plan_walk(int M, int N, int K, int kind, int accumulate, int worker,
  * x fp32 [M, C] (row stride ldx) -> out (bf16 if out_is_bf16 else fp32; row stride ldo, so it can be a column
  * slice of the [M, 4C] decoder input, models_painter.py:422); mean/rstd [M] saved for backward (nullable).
  * bwd: dx = LN'(dy) (+ dres); dgamma/dbeta += column sums (caller initialises; deterministic two-stage
- * reduction through `workspace`).                                                                         */
+ * reduction through `workspace`).  dgamma = dbeta = NULL (frozen affine parameters): no reduction, `workspace`
+ * may be NULL, dx is bit-identical.  In the _cast form each of dgamma, dbeta and colsum may be NULL on its own (that
+ * sum is skipped; with all three NULL `workspace` may be NULL); dx and dx_bf16 are bit-identical.             */
 int pk_layernorm_fwd(const float* x, int ldx, const float* gamma, const float* beta, float eps, void* out,
                      int ldo, int out_is_bf16, float* mean, float* rstd, int M, int C, void* stream);
 long long pk_layernorm_bwd_ws_floats(int M, int C); /* fp32 elements of `workspace` (per-block partial sums) */
@@ -99,11 +101,18 @@ int pk_layernorm_bwd(const void* dy, int dy_is_bf16, int lddy, const float* x, i
  * patches of imgs then tgts, bf16 [2*B*h*w, Cin*p*p]; the conv itself is pk_gemm_bf16 on these rows.       */
 int pk_im2col_patch(const float* imgs, const float* tgts, void* out_bf16, int B, int Cin, int H, int W, int p,
                     void* stream);
+/* Input gradient of the PatchEmbed (prompt tuning, saliency): the exact inverse of pk_im2col_patch's layout.
+ * dcols_x / dcols_y fp32 [B*h*w, Cin*p*p] (the patch-embed dgrad dE . W of the x rows / of the y rows; they may be the
+ * two halves of one [2*B*h*w, Cin*p*p] buffer) -> dimgs / dtgts fp32 NCHW [B, Cin, H, W], overwritten.  Either output
+ * may be NULL: its half of the columns is then not read and may be NULL too.                                  */
+int pk_col2im_patch(const float* dcols_x, const float* dcols_y, float* dimgs, float* dtgts, int B, int Cin, int H,
+                    int W, int p, void* stream);
 
 /* Token assembly (models_painter.py:392-409; SegGPT type tokens models_seggpt.py:414-420) and its backward.
  * E fp32 [2B*N, C] (x rows then y rows); mask uint8 [maskB, N] (maskB = 1 broadcasts); pos fp32 [N, C];
  * type_emb fp32 [B, C] or NULL.  bwd: dE bf16 (y rows gated by 1-mask), dpos [N,C], dseg/dmask_token [C]
- * (atomically accumulated, caller zero-initialises).                                                      */
+ * (atomically accumulated, caller zero-initialises).  Frozen parameters: dpos = NULL skips the position gradient,
+ * dseg_x = dseg_y = dmask_token = NULL (all three) skips the token reductions; dE is unchanged.                 */
 int pk_assemble_tokens(const float* E, const uint8_t* mask, int maskB, const float* mask_token,
                        const float* seg_x, const float* seg_y, const float* pos, const float* type_emb,
                        float* out, int B, int N, int C, void* stream);
@@ -141,7 +150,9 @@ int pk_ensemble_resid(const float* a, const float* z, float* out, int G, int P, 
  * 63-125).  qkv bf16 [B*h*w, 3*heads*64] with columns (3, head, 64); th/tw = pk_relpos_table_bf16 outputs
  * (bf16, zero-padded to th_pad/tw_pad rows, multiples of 16); w must divide 112 (2,4,7,8,14,28,56).
  * fwd: out bf16 [B*N, heads*64], lse fp32 [B*heads, N] (log2 domain, nullable).
- * bwd: dqkv bf16 like qkv; dTh [2h-1,64], dTw [2w-1,64] fp32, added to (zero-initialise);
+ * bwd: dqkv bf16 like qkv; dTh [2h-1,64], dTw [2w-1,64] fp32, added to (zero-initialise); dTh = dTw = NULL (frozen
+ *      tables): no table gradients - the dQ kernel leaves out its G^T Q partials, the reduction kernel does not run,
+ *      dt_ws may be NULL - and dqkv is bit-identical;
  *      scratch: delta [B*heads*N], relh_g [B*heads*Np*h], relw_g [B*heads*Np*w] (Np = N rounded up to 128), dt_ws
  *      [pk_attn_bwd_ws_floats(B, heads, h, w)] fp32 (per-CTA partial table gradients, reduced by a
  *      second kernel instead of same-address atomics).                                                     */
@@ -180,9 +191,18 @@ int pk_decoder_head_fwd(const void* g_nhwc, const void* wmat, const float* head_
                         float* num, int B, int H, int W, int p, int loss_kind, void* stream);
 int pk_loss_finalize(const float* stats, const float* num, float* loss, float* coef, int B, int seggpt,
                      void* stream);
+/* pk_decoder_head_bwd: dc1 (bf16 NHWC) and, when dhead_params_zeroed != NULL, the head parameters' gradients added
+ * at offsets 64..386 of it (NULL: frozen head, no reductions; dc1 is bit-identical).
+ * pk_decoder_head_bwd_dtgt: the same kernel, which also stores the loss's gradient with respect to the targets,
+ * dtgts fp32 NCHW [B, 3, H, W] = -dpred = -(gscale * coef[b] * M * valid * dl/dd), d = pred - tgt (exact for
+ * every loss_kind); it does not include the targets' path through the encoder.                               */
 int pk_decoder_head_bwd(const void* c1, const float* tgts, const uint8_t* mask, int maskB, const float* valid,
                         const float* coef, const float* gscale, const float* head_params, void* dc1,
                         float* dhead_params_zeroed, int B, int H, int W, int p, int loss_kind, void* stream);
+int pk_decoder_head_bwd_dtgt(const void* c1, const float* tgts, const uint8_t* mask, int maskB, const float* valid,
+                             const float* coef, const float* gscale, const float* head_params, void* dc1,
+                             float* dhead_params_zeroed, float* dtgts, int B, int H, int W, int p, int loss_kind,
+                             void* stream);
 int pk_conv3x3_dgrad_unshuffle(const void* dc1_nhwc, const void* wmat_t, void* out_tok, int B, int H, int W,
                                int p, void* stream);
 int pk_conv3x3_wgrad(const void* g_nhwc, const void* dc1_nhwc, float* out, int B, int H, int W, void* stream);

@@ -66,7 +66,6 @@ class GradArena:
         self.clean = True            # slab is all zeros
         self.active = False          # a backward is writing into `cur`
         self.sync = None             # dist_utils.GradSync, when data parallel
-        self.handoff = None          # (dx fp32, bf16(scale * dx)) passed from block i+1's backward to block i's
         self._step = None
 
     # ------------------------------------------------------------------ views
@@ -89,7 +88,6 @@ class GradArena:
         if self._step is step_token:
             return self.active
         self._step = step_token
-        self.handoff = None
         accumulating = any(p.grad is not None for p in self.params)
         self.active = True
         if accumulating:
@@ -114,7 +112,6 @@ class GradArena:
     def end_backward(self):
         if self.active and self.sync is not None:
             self.sync.finish(self)
-        self.handoff = None
 
     def mark_clean(self):
         self.clean = True

@@ -613,8 +613,10 @@ attn_fwd_split3_kernel(const SplitAttnArgs a) {
 //   adds it up tile after tile: no atomics, a fixed order, reproducible.  Image-column entries are summed in
 //   registers and stored to drelw_s after the loop; image-row entries are added into drelh_s.
 //   G[q, r] = dRelh[q, i_q + h - 1 - r] for the T_h rows r of the staged tables (zero outside [0, h)), likewise for
-//   T_w; the table-gradient partials of the CTA are G^T Q, ws[cta][c][table row].
+//   T_w; the table-gradient partials of the CTA are G^T Q, ws[cta][c][table row].  TGRAD = false (frozen rel-pos
+//   tables) leaves those partials out; dQ is computed by the same instructions in the same order either way.
 // smem: sQ | sdO | K/V ring (tables after the loop) | E | relh_s | relw_s | drelh_s | drelw_s
+template <bool TGRAD>
 __global__ void __launch_bounds__(AT_THREADS)
 attn_bwd_dq_kernel(const AttnArgs a) {
   extern __shared__ uint8_t smem_raw[];
@@ -863,6 +865,7 @@ attn_bwd_dq_kernel(const AttnArgs a) {
     }
   }
 
+  if constexpr (!TGRAD) return;
   // table-gradient partials of this CTA, G^T Q in 64-row chunks of the staged table rows (every entry of the slice
   // is written; queries past N contribute nothing)
   const int rows = Lh + Lw;
@@ -1201,7 +1204,8 @@ extern "C" int pk_attn_fwd_split3(const float* qkv, const float* th, const float
 // scratch buffers (caller-allocated): delta [B*heads*N], relh_g [B*heads*Np*h], relw_g [B*heads*Np*w] fp32 with
 // Np = N rounded up to a multiple of 128 (query-major rows of bias values)
 // dt_ws: pk_attn_bwd_ws_floats(B, heads, h, w) fp32 (per-CTA partial table gradients)
-// dTh [2h-1, 64], dTw [2w-1, 64]: fp32, ADDED to (caller zero-initialises or passes a running gradient)
+// dTh [2h-1, 64], dTw [2w-1, 64]: fp32, ADDED to (caller zero-initialises or passes a running gradient); both NULL:
+// no table gradients (the dQ kernel skips its G^T Q partials, no reduction runs, dt_ws may be NULL), dqkv unchanged
 extern "C" long long pk_attn_bwd_ws_floats(int B, int heads, int h, int w) {
   const long long ctas = static_cast<long long>((h * w + AT_BM - 1) / AT_BM) * heads * B;
   return ctas * (2 * h - 1 + 2 * w - 1) * 64;
@@ -1212,7 +1216,11 @@ static int attn_bwd_impl(const void* qkv, const void* O, const void* dO, const f
                          float* relw_g, float* dt_ws, int B, int heads, int h, int w, int th_pad, int tw_pad,
                          int rel_ready, void* stream) {
   if (attn_check(qkv, th, tw, B, heads, h, w, th_pad, tw_pad, "pk_attn_bwd")) return 1;
-  PK_CHECK(O && dO && lse && dqkv && dTh && dTw && delta && relh_g && relw_g && dt_ws, "pk_attn_bwd: null pointer");
+  PK_CHECK(O && dO && lse && dqkv && delta && relh_g && relw_g, "pk_attn_bwd: null pointer");
+  // dTh = dTw = NULL: the tables' gradients are not needed (frozen tables); dt_ws is then unused and may be NULL
+  const bool tgrad = dTh != nullptr;
+  PK_CHECK((dTw != nullptr) == tgrad, "pk_attn_bwd: dTh and dTw must both be given or both be NULL");
+  PK_CHECK(!tgrad || dt_ws, "pk_attn_bwd: null pointer (dt_ws)");
   AttnArgs a = attn_args(qkv, th, tw, B, heads, h, w);
   a.O = static_cast<const __nv_bfloat16*>(O);
   a.dO = static_cast<const __nv_bfloat16*>(dO);
@@ -1237,7 +1245,7 @@ static int attn_bwd_impl(const void* qkv, const void* O, const void* dO, const f
                static_cast<const __nv_bfloat16*>(O), static_cast<const __nv_bfloat16*>(dO), delta, B, N, heads);
     PK_LAUNCH_CHECK("pk_attn_bwd(delta)");
   }
-  if (launch_attn(attn_bwd_dq_kernel, grid,
+  if (launch_attn(tgrad ? attn_bwd_dq_kernel<true> : attn_bwd_dq_kernel<false>, grid,
                   1024 + 3 * AT_TILE + kv_ring_bytes(h, w) + 2 * rel_bytes, st, a,
                   "pk_attn_bwd(dq)"))
     return 2;
@@ -1249,7 +1257,7 @@ static int attn_bwd_impl(const void* qkv, const void* O, const void* dO, const f
                     "pk_attn_bwd(dkv)"))
       return 2;
   }
-  {
+  if (tgrad) {
     const int rows = 2 * h - 1 + 2 * w - 1;
     const int nctas = static_cast<int>(grid.x * grid.y * grid.z);
     launch_pdl(attn_dt_reduce_kernel, dim3(64, DT_STRIPES, (rows + DT_RX - 1) / DT_RX), dim3(DT_RX, DT_RY), 0, st,

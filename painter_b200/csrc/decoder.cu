@@ -263,6 +263,10 @@ head_bwd_kernel(const __nv_bfloat16* __restrict__ c1, const float* __restrict__ 
 // transpose-reduce (30 shuffles per quantity: afterwards lane l holds channels 32 (l & 1) + 2 (l >> 1) + {0, 1} summed
 // over the warp's pixels).  Head parameters are staged once per block in shared memory as {gamma, beta, w0, w1}, {w2}
 // records (two broadcast LDS.128 per channel); no global or __constant__ state.
+// PARAMS = false (frozen head): no parameter-gradient reductions.  DTGT: also stores the loss's target gradient
+// dtgts = -dpred when dtgts != NULL (fp32 NCHW; every loss_kind is a function of pred - tgt).  dc1 is the same in every
+// instantiation.  The frozen head has one instantiation, <false, true>, which also serves dtgts = NULL: without the
+// stores, or without the register fence on ge[] below, ptxas schedules the frozen form into 255 registers and spills.
 // ---------------------------------------------------------------------------------------------
 // v[32] per lane, reduced over the 16 lanes of equal parity; result v[0], v[1] (see above)
 __device__ __forceinline__ void transpose_reduce_pairs(float (&v)[32], int lane) {
@@ -291,12 +295,13 @@ __device__ __forceinline__ float lds_f(uint32_t addr) {
   return v;
 }
 
+template <bool PARAMS, bool DTGT>
 __global__ void __launch_bounds__(128, 2)
 head_bwd2_kernel(const __nv_bfloat16* __restrict__ c1, const float* __restrict__ tgts,
                  const uint8_t* __restrict__ mask, int maskB, const float* __restrict__ valid,
                  const float* __restrict__ coef, const float* __restrict__ gscale, const float* __restrict__ hp,
-                 __nv_bfloat16* __restrict__ dc1, float* __restrict__ dhp, int B, int H, int W, int p, int loss_kind,
-                 int pix_per_warp) {
+                 __nv_bfloat16* __restrict__ dc1, float* __restrict__ dhp, float* __restrict__ dtgts, int B, int H,
+                 int W, int p, int loss_kind, int pix_per_warp) {
   __shared__ float4 prm[64][2];     // [k] = {gamma, beta, w0, w1}, {w2, -, -, -}
   __shared__ float red[4][323];
   const int lane = threadIdx.x & 31, wq = threadIdx.x >> 5;
@@ -378,21 +383,33 @@ head_bwd2_kernel(const __nv_bfloat16* __restrict__ c1, const float* __restrict__
         dp[c] = cf * vl[c] * dl;
       }
     }
-    if (hsel == 0) {
-      db0 += dp[0];
-      db1v += dp[1];
-      db2 += dp[2];
+    if constexpr (DTGT) {
+      if (dtgts != nullptr && live && hsel == 0) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) dtgts[(static_cast<size_t>(bq) * 3 + c) * plane + yx] = -dp[c];
+      }
+    }
+    float t[32];
+    if constexpr (PARAMS) {
+      if (hsel == 0) {
+        db0 += dp[0];
+        db1v += dp[1];
+        db2 += dp[2];
+      }
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {      // dW_c[k] += dp_c * gelu(ln_k)
+#pragma unroll
+        for (int j = 0; j < 32; ++j) t[j] = ge[j] * dp[c];
+        transpose_reduce_pairs(t, lane);
+        acc[2 + c][0] += t[0];
+        acc[2 + c][1] += t[1];
+      }
+    }
+    if constexpr (!PARAMS) {   // see above: keeps the frozen form at 189 registers, no spill
+#pragma unroll
+      for (int j = 0; j < 32; ++j) asm volatile("" : "+f"(ge[j])::"memory");
     }
     // ---- backward through 1x1, GELU, LayerNorm2D
-    float t[32];
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {      // dW_c[k] += dp_c * gelu(ln_k)
-#pragma unroll
-      for (int j = 0; j < 32; ++j) t[j] = ge[j] * dp[c];
-      transpose_reduce_pairs(t, lane);
-      acc[2 + c][0] += t[0];
-      acc[2 + c][1] += t[1];
-    }
     float dln[32];
     float a1 = 0.f, a2 = 0.f;
 #pragma unroll
@@ -407,14 +424,16 @@ head_bwd2_kernel(const __nv_bfloat16* __restrict__ c1, const float* __restrict__
       a2 += dx * xh;
       t[j] = d * xh;
     }
-    transpose_reduce_pairs(t, lane);    // dgamma
-    acc[0][0] += t[0];
-    acc[0][1] += t[1];
+    if constexpr (PARAMS) {
+      transpose_reduce_pairs(t, lane);    // dgamma
+      acc[0][0] += t[0];
+      acc[0][1] += t[1];
 #pragma unroll
-    for (int j = 0; j < 32; ++j) t[j] = dln[j];
-    transpose_reduce_pairs(t, lane);    // dbeta
-    acc[1][0] += t[0];
-    acc[1][1] += t[1];
+      for (int j = 0; j < 32; ++j) t[j] = dln[j];
+      transpose_reduce_pairs(t, lane);    // dbeta
+      acc[1][0] += t[0];
+      acc[1][1] += t[1];
+    }
     a1 = pair_sum(a1) * (1.f / 64);
     a2 = pair_sum(a2) * (1.f / 64);
     if (live) {
@@ -434,6 +453,7 @@ head_bwd2_kernel(const __nv_bfloat16* __restrict__ c1, const float* __restrict__
     }
 #undef HB2_X
   }
+  if constexpr (!PARAMS) return;
   db0 = warp_sum(db0);
   db1v = warp_sum(db1v);
   db2 = warp_sum(db2);
@@ -495,19 +515,19 @@ extern "C" int pk_loss_finalize(const float* stats, const float* num, float* los
 static int g_head_bwd_legacy = 0;
 // test hook: 1 = the warp-per-pixel kernel of round 1 (kept as an independent implementation to cross-check)
 extern "C" void pk_head_bwd_legacy(int on) { g_head_bwd_legacy = on; }
-extern "C" int pk_decoder_head_bwd(const void* c1, const float* tgts, const uint8_t* mask, int maskB,
-                                   const float* valid, const float* coef, const float* gscale,
-                                   const float* head_params, void* dc1, float* dhead_params_zeroed, int B,
-                                   int H, int W, int p, int loss_kind, void* stream) {
-  PK_CHECK(c1 && tgts && mask && valid && coef && head_params && dc1 && dhead_params_zeroed,
-           "pk_decoder_head_bwd: null pointer");
+
+static int head_bwd_impl(const void* c1, const float* tgts, const uint8_t* mask, int maskB, const float* valid,
+                         const float* coef, const float* gscale, const float* head_params, void* dc1, float* dhp,
+                         float* dtgts, int B, int H, int W, int p, int loss_kind, void* stream, const char* who) {
+  PK_CHECK(c1 && tgts && mask && valid && coef && head_params && dc1, "%s: null pointer", who);
   PK_CHECK(W % 4 == 0 && static_cast<long long>(B) * H * W < (1ll << 31),
-           "pk_decoder_head_bwd: W must be a multiple of 4 and B*H*W < 2^31");
+           "%s: W must be a multiple of 4 and B*H*W < 2^31", who);
   if (g_head_bwd_legacy) {
+    PK_CHECK(dhp && !dtgts, "%s: the legacy kernel computes the parameter gradients only", who);
     const int grid = sm_count() * 4;
     head_bwd_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
         static_cast<const __nv_bfloat16*>(c1), tgts, mask, maskB, valid, coef, gscale, head_params,
-        static_cast<__nv_bfloat16*>(dc1), dhead_params_zeroed, B, H, W, p, loss_kind);
+        static_cast<__nv_bfloat16*>(dc1), dhp, B, H, W, p, loss_kind);
   } else {
     // a lane pair per pixel; every warp walks `ppw` consecutive pixels (a multiple of 16) so that the block-level
     // parameter-gradient atomics stay ~4 per SM-resident block
@@ -517,10 +537,29 @@ extern "C" int pk_decoder_head_bwd(const void* c1, const float* tgts, const uint
     ppw = (ppw + 15) / 16 * 16;
     const long long warps = (npix + ppw - 1) / ppw;
     const int grid = static_cast<int>((warps + 3) / 4);
-    head_bwd2_kernel<<<grid, 128, 0, static_cast<cudaStream_t>(stream)>>>(
+    auto kernel = dhp ? (dtgts ? head_bwd2_kernel<true, true> : head_bwd2_kernel<true, false>)
+                      : head_bwd2_kernel<false, true>;
+    kernel<<<grid, 128, 0, static_cast<cudaStream_t>(stream)>>>(
         static_cast<const __nv_bfloat16*>(c1), tgts, mask, maskB, valid, coef, gscale, head_params,
-        static_cast<__nv_bfloat16*>(dc1), dhead_params_zeroed, B, H, W, p, loss_kind, static_cast<int>(ppw));
+        static_cast<__nv_bfloat16*>(dc1), dhp, dtgts, B, H, W, p, loss_kind, static_cast<int>(ppw));
   }
-  PK_LAUNCH_CHECK("pk_decoder_head_bwd");
+  PK_LAUNCH_CHECK(who);
   return 0;
+}
+
+extern "C" int pk_decoder_head_bwd(const void* c1, const float* tgts, const uint8_t* mask, int maskB,
+                                   const float* valid, const float* coef, const float* gscale,
+                                   const float* head_params, void* dc1, float* dhead_params_zeroed, int B,
+                                   int H, int W, int p, int loss_kind, void* stream) {
+  return head_bwd_impl(c1, tgts, mask, maskB, valid, coef, gscale, head_params, dc1, dhead_params_zeroed, nullptr, B,
+                       H, W, p, loss_kind, stream, "pk_decoder_head_bwd");
+}
+
+extern "C" int pk_decoder_head_bwd_dtgt(const void* c1, const float* tgts, const uint8_t* mask, int maskB,
+                                        const float* valid, const float* coef, const float* gscale,
+                                        const float* head_params, void* dc1, float* dhead_params_zeroed,
+                                        float* dtgts, int B, int H, int W, int p, int loss_kind, void* stream) {
+  PK_CHECK(dtgts, "pk_decoder_head_bwd_dtgt: null pointer (dtgts)");
+  return head_bwd_impl(c1, tgts, mask, maskB, valid, coef, gscale, head_params, dc1, dhead_params_zeroed, dtgts, B,
+                       H, W, p, loss_kind, stream, "pk_decoder_head_bwd_dtgt");
 }

@@ -167,7 +167,9 @@ ln_bwd_kernel(const void* __restrict__ dy_, int lddy, const float* __restrict__ 
       }
     }
   }
-  // per-block partials, one row of the workspace per block (no atomics: a second small kernel sums the rows)
+  // per-block partials, one row of the workspace per block (no atomics: a second small kernel sums the rows); no
+  // workspace when none of the column sums is wanted
+  if (partials == nullptr) return;
   constexpr int NP = FUSE ? 3 : 2;
   float4* pg = reinterpret_cast<float4*>(partials + static_cast<size_t>(blockIdx.x) * NP * C);
   pg[tid] = ag;
@@ -176,7 +178,8 @@ ln_bwd_kernel(const void* __restrict__ dy_, int lddy, const float* __restrict__ 
 }
 
 // dgamma[c] += sum_b partials[b][c];  dbeta[c] += sum_b partials[b][C + c].   block (32, 8): 32 columns, the
-// rows strided over threadIdx.y, 4 loads in flight per thread.
+// rows strided over threadIdx.y, 4 loads in flight per thread.  A block whose target is NULL (a gradient that is not
+// needed) does nothing: C % 128 == 0 keeps each block's 32 columns inside one target.
 __global__ void __launch_bounds__(256)
 ln_bwd_reduce_kernel(const float* __restrict__ partials, int nblocks, float* __restrict__ dgamma,
                      float* __restrict__ dbeta, float* __restrict__ colsum, int C, int np) {
@@ -184,6 +187,8 @@ ln_bwd_reduce_kernel(const float* __restrict__ partials, int nblocks, float* __r
   pdl_launch_dependents();   // programmatic dependent launch (host_common.h)
   pdl_wait();
   const int c = blockIdx.x * 32 + threadIdx.x;
+  const int seg = blockIdx.x * 32 / C;
+  if ((seg == 0 ? dgamma : seg == 1 ? dbeta : colsum) == nullptr) return;
   const size_t ld = static_cast<size_t>(np) * C;
   float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
   int b = threadIdx.y;
@@ -235,6 +240,34 @@ im2col_patch_kernel(const float* __restrict__ imgs, const float* __restrict__ tg
     u.x = pack_bf16x2(a.x, a.y); u.y = pack_bf16x2(a.z, a.w);
     u.z = pack_bf16x2(b.x, b.y); u.w = pack_bf16x2(b.z, b.w);
     *reinterpret_cast<uint4*>(out + row * kdim + k0) = u;
+  }
+}
+
+// Input gradient of the PatchEmbed lowering: the exact inverse of im2col_patch_kernel's layout (the patches do not
+// overlap, so every image element is one entry of the column matrix).  dcols_x / dcols_y fp32 [B*h*w, Cin*p*p] (the
+// x rows and the y rows) -> dimgs / dtgts fp32 NCHW; a NULL half is neither read nor written (img0 / nimg select the
+// images).  thread = 4 consecutive pixels of one image row (p % 8 == 0 keeps them inside one patch).
+__global__ void __launch_bounds__(256)
+col2im_patch_kernel(const float* __restrict__ dcols_x, const float* __restrict__ dcols_y, float* __restrict__ dimgs,
+                    float* __restrict__ dtgts, int B, int Cin, int H, int W, int p, int img0, int nimg) {
+  const int h = H / p, w = W / p, N = h * w;
+  const int kdim = Cin * p * p, w4 = W / 4;
+  const size_t per_img = static_cast<size_t>(Cin) * H * w4;
+  const size_t total = static_cast<size_t>(nimg) * per_img;
+  for (size_t idx = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; idx < total;
+       idx += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const int img = img0 + static_cast<int>(idx / per_img);
+    const size_t e = idx % per_img;
+    const int x = static_cast<int>(e % w4) * 4;
+    const size_t cy = e / w4;
+    const int y = static_cast<int>(cy % H), c = static_cast<int>(cy / H);
+    const int i = y / p, r = y % p, j = x / p, s = x % p;
+    const int b = img < B ? img : img - B;
+    const float4 v = *reinterpret_cast<const float4*>((img < B ? dcols_x : dcols_y) +
+                                                      (static_cast<size_t>(b) * N + i * w + j) * kdim +
+                                                      (c * p + r) * p + s);
+    float* dst = (img < B ? dimgs : dtgts) + static_cast<size_t>(b) * Cin * H * W;
+    *reinterpret_cast<float4*>(dst + cy * W + x) = v;
   }
 }
 
@@ -304,9 +337,11 @@ __global__ void assemble_bwd_kernel(const float* __restrict__ dZ, const uint8_t*
       u.y = pack_bf16x2(d.z, d.w);
       reinterpret_cast<uint2*>(dE)[off] = u;
     }
-    reinterpret_cast<float4*>(dpos)[static_cast<size_t>(n) * c4n + c4] =
-        make_float4(sx.x + sy.x, sx.y + sy.y, sx.z + sy.z, sx.w + sy.w);
+    if (dpos)
+      reinterpret_cast<float4*>(dpos)[static_cast<size_t>(n) * c4n + c4] =
+          make_float4(sx.x + sy.x, sx.y + sy.y, sx.z + sy.z, sx.w + sy.w);
   }
+  if (dseg_x == nullptr) return;   // frozen tokens: no reduction (the host passes all three or none)
   const int TY = blockDim.y;
   sred[(0 * TY + threadIdx.y) * c4n + c4] = sx;
   sred[(1 * TY + threadIdx.y) * c4n + c4] = sy;
@@ -563,9 +598,13 @@ extern "C" long long pk_layernorm_bwd_ws_floats(int M, int C) {
 extern "C" int pk_layernorm_bwd(const void* dy, int dy_is_bf16, int lddy, const float* x, int ldx, const float* mean,
                                 const float* rstd, const float* gamma, const float* dres, float* dx,
                                 float* dgamma, float* dbeta, float* workspace, int M, int C, void* stream) {
-  PK_CHECK(dy && x && mean && rstd && gamma && dx && dgamma && dbeta && workspace, "pk_layernorm_bwd: null pointer");
+  PK_CHECK(dy && x && mean && rstd && gamma && dx, "pk_layernorm_bwd: null pointer");
+  // dgamma = dbeta = NULL: no affine gradients (frozen LayerNorm); no workspace is touched and dx is unchanged
+  const bool affine = dgamma || dbeta;
+  PK_CHECK(!affine || workspace, "pk_layernorm_bwd: null pointer (workspace)");
   PK_CHECK(C % 128 == 0 && C <= 1024 && lddy % 4 == 0 && ldx % 4 == 0, "pk_layernorm_bwd: bad C=%d", C);
   const int grid = ln_bwd_grid(M);
+  if (!affine) workspace = nullptr;
   if (dy_is_bf16)
     launch_pdl(ln_bwd_kernel<false, true>, dim3(grid), dim3(C / 4), 0, static_cast<cudaStream_t>(stream), dy, lddy, x,
                ldx, mean, rstd, gamma, dres, dx, workspace, M, C, static_cast<const float*>(nullptr), 0,
@@ -575,9 +614,11 @@ extern "C" int pk_layernorm_bwd(const void* dy, int dy_is_bf16, int lddy, const 
                ldx, mean, rstd, gamma, dres, dx, workspace, M, C, static_cast<const float*>(nullptr), 0,
                static_cast<__nv_bfloat16*>(nullptr));
   PK_LAUNCH_CHECK("pk_layernorm_bwd");
-  launch_pdl(ln_bwd_reduce_kernel, dim3(2 * C / 32), dim3(32, 8), 0, static_cast<cudaStream_t>(stream),
-             static_cast<const float*>(workspace), grid, dgamma, dbeta, static_cast<float*>(nullptr), C, 2);
-  PK_LAUNCH_CHECK("pk_layernorm_bwd(reduce)");
+  if (affine) {
+    launch_pdl(ln_bwd_reduce_kernel, dim3(2 * C / 32), dim3(32, 8), 0, static_cast<cudaStream_t>(stream),
+               static_cast<const float*>(workspace), grid, dgamma, dbeta, static_cast<float*>(nullptr), C, 2);
+    PK_LAUNCH_CHECK("pk_layernorm_bwd(reduce)");
+  }
   return 0;
 }
 
@@ -587,8 +628,12 @@ extern "C" int pk_layernorm_bwd_cast(const void* dy, int dy_is_bf16, int lddy, c
                                      const float* rstd, const float* gamma, const float* dres, float* dx,
                                      float* dgamma, float* dbeta, float* workspace, const float* rowscale,
                                      int rows_per_group, void* dx_bf16, float* colsum, int M, int C, void* stream) {
-  PK_CHECK(dy && x && mean && rstd && gamma && dx && dgamma && dbeta && workspace && dx_bf16 && colsum,
-           "pk_layernorm_bwd_cast: null pointer");
+  PK_CHECK(dy && x && mean && rstd && gamma && dx && dx_bf16, "pk_layernorm_bwd_cast: null pointer");
+  // dgamma / dbeta / colsum = NULL: that column sum is not needed; with all three NULL no workspace is touched.  dx and
+  // dx_bf16 are unchanged either way.
+  const bool sums = dgamma || dbeta || colsum;
+  PK_CHECK(!sums || workspace, "pk_layernorm_bwd_cast: null pointer (workspace)");
+  if (!sums) workspace = nullptr;
   PK_CHECK(C % 128 == 0 && C <= 1024 && lddy % 4 == 0 && ldx % 4 == 0, "pk_layernorm_bwd_cast: bad C=%d", C);
   if (rowscale) PK_CHECK(rows_per_group > 0, "pk_layernorm_bwd_cast: rows_per_group must be > 0");
   int grid = sm_count() * 2;   // the fused variant keeps 2 blocks per SM resident (<= ln_bwd_grid(M): workspace fits)
@@ -602,9 +647,11 @@ extern "C" int pk_layernorm_bwd_cast(const void* dy, int dy_is_bf16, int lddy, c
                ldx, mean, rstd, gamma, dres, dx, workspace, M, C, rowscale, rows_per_group,
                static_cast<__nv_bfloat16*>(dx_bf16));
   PK_LAUNCH_CHECK("pk_layernorm_bwd_cast");
-  launch_pdl(ln_bwd_reduce_kernel, dim3(3 * C / 32), dim3(32, 8), 0, static_cast<cudaStream_t>(stream),
-             static_cast<const float*>(workspace), grid, dgamma, dbeta, colsum, C, 3);
-  PK_LAUNCH_CHECK("pk_layernorm_bwd_cast(reduce)");
+  if (sums) {
+    launch_pdl(ln_bwd_reduce_kernel, dim3(3 * C / 32), dim3(32, 8), 0, static_cast<cudaStream_t>(stream),
+               static_cast<const float*>(workspace), grid, dgamma, dbeta, colsum, C, 3);
+    PK_LAUNCH_CHECK("pk_layernorm_bwd_cast(reduce)");
+  }
   return 0;
 }
 
@@ -616,6 +663,19 @@ extern "C" int pk_im2col_patch(const float* imgs, const float* tgts, void* out_b
   im2col_patch_kernel<<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       imgs, tgts, static_cast<__nv_bfloat16*>(out_bf16), B, Cin, H, W, p);
   PK_LAUNCH_CHECK("pk_im2col_patch");
+  return 0;
+}
+
+extern "C" int pk_col2im_patch(const float* dcols_x, const float* dcols_y, float* dimgs, float* dtgts, int B, int Cin,
+                               int H, int W, int p, void* stream) {
+  PK_CHECK((dcols_x || !dimgs) && (dcols_y || !dtgts), "pk_col2im_patch: null pointer");
+  PK_CHECK(p % 8 == 0 && H % p == 0 && W % p == 0 && W % 4 == 0, "pk_col2im_patch: bad geometry");
+  const int img0 = dimgs ? 0 : B, nimg = (dimgs ? B : 0) + (dtgts ? B : 0);
+  if (nimg == 0) return 0;
+  const size_t total = static_cast<size_t>(nimg) * Cin * H * (W / 4);
+  col2im_patch_kernel<<<grid_for(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      dcols_x, dcols_y, dimgs, dtgts, B, Cin, H, W, p, img0, nimg);
+  PK_LAUNCH_CHECK("pk_col2im_patch");
   return 0;
 }
 
@@ -634,8 +694,11 @@ extern "C" int pk_assemble_tokens(const float* E, const uint8_t* mask, int maskB
 extern "C" int pk_assemble_tokens_bwd(const float* dZ, const uint8_t* mask, int maskB, void* dE_bf16,
                                       float* dpos, float* dseg_x, float* dseg_y, float* dmask_token, int B,
                                       int N, int C, void* stream) {
-  PK_CHECK(dZ && mask && dE_bf16 && dpos && dseg_x && dseg_y && dmask_token,
-           "pk_assemble_tokens_bwd: null pointer");
+  // dpos = NULL: the position gradient is not needed; dseg_x = dseg_y = dmask_token = NULL: the token gradients are
+  // not needed (all three or none).  dE is unchanged either way.
+  PK_CHECK(dZ && mask && dE_bf16, "pk_assemble_tokens_bwd: null pointer");
+  PK_CHECK((dseg_x != nullptr) == (dseg_y != nullptr) && (dseg_x != nullptr) == (dmask_token != nullptr),
+           "pk_assemble_tokens_bwd: dseg_x, dseg_y and dmask_token must all be given or all be NULL");
   PK_CHECK(C % 4 == 0 && C / 4 <= 256, "pk_assemble_tokens_bwd: C=%d unsupported", C);
   const int tx = C / 4;
   int ty = 1024 / tx;

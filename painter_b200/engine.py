@@ -17,14 +17,24 @@ from .ops import EPI_BF16, EPI_DGELU, EPI_F32, EPI_GELU, EPI_PIXSHUF, EPI_RESID
 LOSS_KINDS = {"smoothl1": 0, "l1": 1, "l2": 2, "l1l2": 3}
 
 
-class StageEnv:
-    """Per-forward bookkeeping handed to every stage (non-tensor argument): the module's gradient arena, a token that
-    identifies the step, the stage's arena group name and its parameters by role, and - for a block - the hand-off to
-    the block below it in the stack (whose MLP branch consumes this block's dx)."""
-    __slots__ = ("arena", "token", "name", "prm", "below")
+class StepLink:
+    """State the block backwards of one forward share: the hand-off (dx fp32, bf16(scale * dx)) that block i+1's LN1
+    backward passes to block i's MLP branch."""
+    __slots__ = ("handoff",)
 
-    def __init__(self, arena, token, name, prm, below=None):
-        self.arena, self.token, self.name, self.prm, self.below = arena, token, name, prm, below
+    def __init__(self):
+        self.handoff = None
+
+
+class StageEnv:
+    """Per-forward bookkeeping handed to every stage (non-tensor argument): the module's gradient arena (None: no
+    parameter requires grad), a token that identifies the step, the stage's arena group name and its parameters by
+    role, and - for a block - the block below it in the stack (whose MLP branch consumes this block's dx) and the
+    forward's StepLink that carries the hand-off."""
+    __slots__ = ("arena", "token", "name", "prm", "below", "link")
+
+    def __init__(self, arena, token, name, prm, below=None, link=None):
+        self.arena, self.token, self.name, self.prm, self.below, self.link = arena, token, name, prm, below, link
 
     def begin(self):
         """True if this backward writes parameter gradients into the arena."""
@@ -100,13 +110,18 @@ def resize_rel_table(table, size):
 
 
 class EmbedFn(torch.autograd.Function):
+    """imgs, tgts fp32 NCHW -> tokens [2B*N, C].  Gradients flow to imgs / tgts (prompt tuning, saliency) through the
+    patch-embed dgrad and pk_col2im_patch; every parameter gradient is computed only if that parameter requires grad
+    (the weight gradient's operand `cols` is not even saved when the weight is frozen)."""
+
     @staticmethod
     def forward(ctx, imgs, tgts, mask_u8, type_emb, Wp, bp, mask_token, seg_x, seg_y, pos_embed, p, has_cls, env):
         B, Cin, H, W = imgs.shape
         h, w = H // p, W // p
         N, C = h * w, Wp.shape[0]
         cols = ops.im2col_patch(imgs, tgts, p)
-        E = ops.gemm(cols, bf16_weight(Wp, (C, Cin * p * p)), kind=EPI_F32, bias=bp)
+        wp = bf16_weight(Wp, (C, Cin * p * p))
+        E = ops.gemm(cols, wp, kind=EPI_F32, bias=bp)
         pe = pos_embed[0, 1:] if has_cls else pos_embed[0]
         s = int(round(pe.shape[0] ** 0.5))
         assert s * s == pe.shape[0]
@@ -114,46 +129,68 @@ class EmbedFn(torch.autograd.Function):
         pos = pe if (s == h and s == w) else ops.bicubic_fwd(pe.view(s, s, C), h, w).view(N, C)
         z = ops.assemble_tokens(E, mask_u8, mask_token.reshape(C).contiguous(), seg_x.reshape(C).contiguous(),
                                 seg_y.reshape(C).contiguous(), pos, type_emb, B, N, C)
-        ctx.save_for_backward(cols, mask_u8)
-        ctx.meta = (B, N, C, h, w, s, has_cls, Wp.shape, pos_embed.shape, mask_token.shape, type_emb is not None)
+        need = ctx.needs_input_grad
+        ctx.save_for_backward(cols if need[4] else None, mask_u8, wp if (need[0] or need[1]) else None)
+        ctx.meta = (B, N, C, h, w, s, has_cls, Wp.shape, pos_embed.shape, mask_token.shape, type_emb is not None,
+                    (Cin, H, W, p))
         ctx.env = env
         return z
 
     @staticmethod
     def backward(ctx, dz):
-        cols, mask_u8 = ctx.saved_tensors
-        B, N, C, h, w, s, has_cls, wshape, pshape, tshape, has_type = ctx.meta
-        if has_type and ctx.needs_input_grad[3]:
+        cols, mask_u8, wp = ctx.saved_tensors
+        B, N, C, h, w, s, has_cls, wshape, pshape, tshape, has_type, (Cin, H, W, p) = ctx.meta
+        need = ctx.needs_input_grad
+        if has_type and need[3]:
             raise NotImplementedError("painter_b200: gradients of the SegGPT type tokens are not implemented "
                                       "(SegGPT is an inference path, seggpt_engine.py:26)")
         env = ctx.env
         act = env is not None and env.begin()
         dz = dz.contiguous()
-        if act:
-            g = {k: env.grad(True, k) for k in ("w", "b", "mt", "sx", "sy", "pe")}
-            tok = (g["sx"].view(C), g["sy"].view(C), g["mt"].view(C))
-        else:
-            g, tok = None, None
-        dE, dpos, dsx, dsy, dmt = ops.assemble_tokens_bwd(dz, mask_u8, B, N, C, token_grads=tok)
-        dW = _wgrad(dE, cols, out=g["w"].view(wshape[0], -1) if act else None).view(wshape)
-        db = ops.colsum_bf16(dE, out=g["b"] if act else None)
-        dpe = g["pe"] if act else torch.zeros(pshape, dtype=torch.float32, device=dz.device)
-        off = 1 if has_cls else 0
-        if s == h and s == w:
-            dpe[0, off:] = dpos
-        else:
-            ops.bicubic_bwd(dpos.view(h, w, C), s, s, out=dpe[0, off:].view(s, s, C))
+        need_tok = need[6] or need[7] or need[8]
+        tok = tuple(env.grad(True, k).view(C) for k in ("sx", "sy", "mt")) if act and need_tok else None
+        dE, dpos, dsx, dsy, dmt = ops.assemble_tokens_bwd(dz, mask_u8, B, N, C, token_grads=tok, want_tokens=need_tok,
+                                                          want_pos=need[9])
+        dW = _wgrad(dE, cols, out=env.grad(True, "w").view(wshape[0], -1) if act else None).view(wshape) \
+            if need[4] else None
+        db = ops.colsum_bf16(dE, out=env.grad(True, "b") if act else None) if need[5] else None
+        dpe = None
+        if need[9]:
+            dpe = env.grad(True, "pe") if act else torch.zeros(pshape, dtype=torch.float32, device=dz.device)
+            off = 1 if has_cls else 0
+            if s == h and s == w:
+                dpe[0, off:] = dpos
+            else:
+                ops.bicubic_bwd(dpos.view(h, w, C), s, s, out=dpe[0, off:].view(s, s, C))
+        dimgs = dtgts = None
+        if need[0] or need[1]:
+            # patch-embed dgrad dE . Wp of the wanted halves only (x rows -> imgs, y rows -> tgts), one GEMM over the
+            # rows of both when both are wanted, then the inverse of the im2col layout
+            lo, hi = (0 if need[0] else B * N), (2 * B * N if need[1] else B * N)
+            dcols = ops.gemm(dE[lo:hi], wp, trans_b=True, kind=EPI_F32)
+            dimgs, dtgts = ops.col2im_patch(dcols[:B * N] if need[0] else None,
+                                            dcols[hi - lo - B * N:] if need[1] else None, B, Cin, H, W, p)
         if act:
             env.arena.stage_done(env.name)
             env.arena.end_backward()
-            return (None, None, None, None, dW, db, g["mt"], g["sx"], g["sy"], dpe, None, None, None)
-        return (None, None, None, None, dW, db, dmt.view(tshape), dsx.view(tshape), dsy.view(tshape), dpe, None,
-                None, None)
+            return (dimgs, dtgts, None, None, dW, db, env.grad(True, "mt") if need[6] else None,
+                    env.grad(True, "sx") if need[7] else None, env.grad(True, "sy") if need[8] else None, dpe, None,
+                    None, None)
+        return (dimgs, dtgts, None, None, dW, db, dmt.view(tshape) if need[6] else None,
+                dsx.view(tshape) if need[7] else None, dsy.view(tshape) if need[8] else None, dpe, None, None, None)
+
+
+# BlockFn's parameter inputs (positions 3 .. 16 of its forward) in the order of models_painter.Block.ROLES
+BLOCK_ROLES = ("n1w", "n1b", "rel_h", "rel_w", "qkv_w", "qkv_b", "proj_w", "proj_b", "n2w", "n2b", "fc1_w", "fc1_b",
+               "fc2_w", "fc2_b")
 
 
 class BlockFn(torch.autograd.Function):
     """x [B'*N, C] fp32 -> same.  meta = (Bp, h, w, heads, eps, ens_groups, ens_P, ws); ws > 0 = windowed block
-    (vitdet_utils.window_partition / window_unpartition around the attention, models_painter.py:220-227)."""
+    (vitdet_utils.window_partition / window_unpartition around the attention, models_painter.py:220-227).
+    Every parameter gradient (weight-gradient GEMM, bias column sums, LayerNorm affine reductions, rel-pos table
+    gradients) is computed only if that parameter requires grad, and the activations only the weight gradients read
+    (u, v, hact) are saved only if qkv / fc1 / fc2 weight requires grad; the dx chain is the same either way."""
 
     @staticmethod
     def forward(ctx, x, drop_a, drop_m, n1w, n1b, rel_h, rel_w, qkv_w, qkv_b, proj_w, proj_b, n2w, n2b, fc1_w,
@@ -200,8 +237,10 @@ class BlockFn(torch.autograd.Function):
         v, mean2, rstd2 = ops.layernorm_fwd(x1, n2w, n2b, eps)
         z, hact = ops.gemm(v, wfc1, kind=EPI_GELU, bias=fc1_b)
         x2 = ops.gemm(hact, wfc2, kind=EPI_RESID, bias=fc2_b, aux=x1, rowscale=drop_m, rows_per_group=N)
-        ctx.save_for_backward(x, mean1, rstd1, u, qkv, ao, lse, th, tw, x1, mean2, rstd2, v, z, hact, wqkv, wproj,
-                              wfc1, wfc2, n1w, n2w, drop_a, drop_m, relh, relw)
+        need = ctx.needs_input_grad
+        ctx.save_for_backward(x, mean1, rstd1, u if need[7] else None, qkv, ao, lse, th, tw, x1, mean2, rstd2,
+                              v if need[13] else None, z, hact if need[15] else None, wqkv, wproj, wfc1, wfc2, n1w,
+                              n2w, drop_a, drop_m, relh, relw)
         ctx.meta = meta
         return x2
 
@@ -218,86 +257,109 @@ class BlockFn(torch.autograd.Function):
         dev = x.device
         dx2 = dx2.contiguous()
         H4 = wfc1.shape[0]
-        # Accumulation targets of the block (LN affine grads, bias grads, the four weight gradients the stream-K
-        # GEMMs add into, the rel-pos table gradients): the parameters' slots in the module's zero-initialised
-        # gradient arena, or - gradient accumulation / no arena - ONE zero-filled slab for the block.
+        need = dict(zip(BLOCK_ROLES, ctx.needs_input_grad[3:17]))
+        tables = need["rel_h"] or need["rel_w"]
+        # Accumulation targets of the parameters that require grad (LN affine grads, bias grads, the four weight
+        # gradients the stream-K GEMMs add into, the rel-pos table gradients): their slots in the module's
+        # zero-initialised gradient arena, or - gradient accumulation / no arena - ONE zero-filled slab for the block.
+        # None for a frozen parameter: its reduction is skipped.
         env = ctx.env
         act = env is not None and env.begin()
         Lh, Lw = th_rows(h if ws == 0 else ws), th_rows(w if ws == 0 else ws)
+        shapes = {"n1w": (C,), "n1b": (C,), "rel_h": (Lh, 64), "rel_w": (Lw, 64), "qkv_w": (3 * C, C),
+                  "qkv_b": (3 * C,), "proj_w": (C, C), "proj_b": (C,), "n2w": (C,), "n2b": (C,), "fc1_w": (H4, C),
+                  "fc1_b": (H4,), "fc2_w": (C, H4), "fc2_b": (C,)}
+        if tables:      # the attention kernel produces both table gradients together
+            need_t = dict(need, rel_h=True, rel_w=True)
+        else:
+            need_t = need
+        g = dict.fromkeys(BLOCK_ROLES)
         rel_native = act and env.prm["rel_h"].shape[0] == Lh and env.prm["rel_w"].shape[0] == Lw
         if act:
-            gv = env.arena.view
-            P = env.prm
-            dn1w, dn1b, dn2w, dn2b = gv(P["n1w"]), gv(P["n1b"]), gv(P["n2w"]), gv(P["n2b"])
-            dfc2_b, dproj_b, dfc1_b, dqkv_b = gv(P["fc2_b"]), gv(P["proj_b"]), gv(P["fc1_b"]), gv(P["qkv_b"])
-            g_qkv, g_proj, g_fc1, g_fc2 = gv(P["qkv_w"]), gv(P["proj_w"]), gv(P["fc1_w"]), gv(P["fc2_w"])
-            if rel_native:
-                g_th, g_tw = gv(P["rel_h"]), gv(P["rel_w"])
-            else:   # resized tables: the gradient flows on through autograd's transpose of the linear resize
-                g_th = torch.zeros((Lh, 64), dtype=torch.float32, device=dev)
-                g_tw = torch.zeros((Lw, 64), dtype=torch.float32, device=dev)
-        else:
-            n_small = 4 * C + 2 * C + H4 + 3 * C
-            sizes = [n_small, 3 * C * C, C * C, H4 * C, C * H4, Lh * 64, Lw * 64]
+            # resized tables get slab buffers: their gradient flows on through autograd's transpose of the resize
+            for r in BLOCK_ROLES:
+                if need_t[r] and (rel_native or r not in ("rel_h", "rel_w")):
+                    g[r] = env.arena.view(env.prm[r])
+        pending = [r for r in BLOCK_ROLES if need_t[r] and g[r] is None]
+        if pending:
+            sizes = [int(torch.Size(shapes[r]).numel()) for r in pending]
             slab = torch.zeros(sum(sizes), dtype=torch.float32, device=dev)
-            small, g_qkv, g_proj, g_fc1, g_fc2, g_th, g_tw = torch.split(slab, sizes)
-            g_qkv, g_proj = g_qkv.view(3 * C, C), g_proj.view(C, C)
-            g_fc1, g_fc2 = g_fc1.view(H4, C), g_fc2.view(C, H4)
-            g_th, g_tw = g_th.view(Lh, 64), g_tw.view(Lw, 64)
-            dn1w, dn1b, dn2w, dn2b = small[0:C], small[C:2 * C], small[2 * C:3 * C], small[3 * C:4 * C]
-            dfc2_b, dproj_b = small[4 * C:5 * C], small[5 * C:6 * C]
-            dfc1_b, dqkv_b = small[6 * C:6 * C + H4], small[6 * C + H4:]
+            for r, t in zip(pending, torch.split(slab, sizes)):
+                g[r] = t.view(shapes[r])
         # ---- MLP branch ----
         # bf16(DropPath scale * dx2) and its column sums (fc2 bias gradient) normally arrive from the LN1 backward of
-        # the block above, which produced dx2 (hand-off through the arena); otherwise one pass over dx2 here
-        ho = env.arena.handoff if act else None
+        # the block above, which produced dx2 (hand-off through the step's StepLink); otherwise one pass over dx2 here
+        link = env.link if env is not None else None
+        ho = link.handoff if link is not None else None
         if ho is not None:
-            env.arena.handoff = None
+            link.handoff = None
             if ho[0].data_ptr() != dx2.data_ptr() or ho[0].shape != dx2.shape:
                 raise RuntimeError("painter_b200: gradient hand-off between blocks does not match the incoming grad")
             dy = ho[1]
         else:
-            dy, _ = ops.scale_cast_colsum(dx2, drop_m, N, colsum_out=dfc2_b)
-        dfc2_w = _wgrad(dy, hact, out=g_fc2)
+            dy, _ = ops.scale_cast_colsum(dx2, drop_m, N, want_colsum=need["fc2_b"], colsum_out=g["fc2_b"])
+        if need["fc2_w"]:
+            _wgrad(dy, hact, out=g["fc2_w"])
         dz = ops.gemm(dy, wfc2, trans_b=True, kind=EPI_DGELU, aux=z)
-        ops.colsum_bf16(dz, out=dfc1_b)
-        dfc1_w = _wgrad(dz, v, out=g_fc1)
+        if need["fc1_b"]:
+            ops.colsum_bf16(dz, out=g["fc1_b"])
+        if need["fc1_w"]:
+            _wgrad(dz, v, out=g["fc1_w"])
         # dgrad outputs that feed a LayerNorm backward are written as bf16 (the reference's autocast Linear backward
         # rounds there too): half the store traffic of the GEMM epilogue and of the LN-backward's dy stream
         dv = ops.gemm(dz, wfc1, trans_b=True, kind=EPI_BF16)
         # LN2 backward also emits the attention branch's incoming gradient: bf16(DropPath scale * dx1) + its column sums
-        dx1, da = ops.layernorm_bwd(dv, x1, mean2, rstd2, n2w, dn2w, dn2b, dres=dx2, cast=(drop_a, N, dproj_b))
+        dx1, da = ops.layernorm_bwd(dv, x1, mean2, rstd2, n2w, g["n2w"], g["n2b"], dres=dx2,
+                                    cast=(drop_a, N, g["proj_b"]))
         # ---- attention branch ----
         if ws > 0:
             da = ops.window_partition_bf16(da, Bp, h, w, ws)
             Bw = da.shape[0] // (ws * ws)
-        dproj_w = _wgrad(da, ao, out=g_proj)
+        if need["proj_w"]:
+            _wgrad(da, ao, out=g["proj_w"])
+        # the rest of the chain only as far as something below needs it: dx / LN1 (x or norm1 trainable), then dqkv
+        need_dx = ctx.needs_input_grad[0]
+        need_du = need_dx or need["n1w"] or need["n1b"]
+        if not (need_du or need["qkv_w"] or need["qkv_b"] or tables):
+            if act:
+                env.arena.stage_done(env.name)
+            return (None, None, None, *[g[r] if need[r] else None for r in BLOCK_ROLES], None, None)
         dao = ops.gemm(da, wproj, trans_b=True, kind=EPI_BF16)
+        dT = (g["rel_h"], g["rel_w"]) if tables else None
         if ws > 0:
-            dqkv, dTh, dTw = ops.attn_bwd(qkv, ao, dao, lse, th, tw, Bw, heads, ws, ws, dT_out=(g_th, g_tw), rel=rel)
+            dqkv, _, _ = ops.attn_bwd(qkv, ao, dao, lse, th, tw, Bw, heads, ws, ws, dT_out=dT, rel=rel,
+                                      table_grads=tables)
         else:
-            dqkv, dTh, dTw = ops.attn_bwd(qkv, ao, dao, lse, th, tw, Bp, heads, h, w, dT_out=(g_th, g_tw), rel=rel)
-        ops.colsum_bf16(dqkv, out=dqkv_b)
-        dqkv_w = _wgrad(dqkv, u, out=g_qkv)
-        if ws > 0:
-            du = ops.gemm(dqkv, wqkv, trans_b=True, kind=EPI_F32)
-            du = ops.window_unpartition(du, Bp, h, w, ws)   # gradients at padded tokens are dropped
-        else:
-            du = ops.gemm(dqkv, wqkv, trans_b=True, kind=EPI_BF16)
-        below = env.below if act else None
-        if below is not None:
-            # the block below consumes dx only through bf16(its DropPath scale * dx): emit that (and the fc2 bias
-            # gradient it implies) in the same pass
-            b_fc2_b, b_drop_m, b_N = below
-            dx, dxb = ops.layernorm_bwd(du, x, mean1, rstd1, n1w, dn1w, dn1b, dres=dx1,
-                                        cast=(b_drop_m, b_N, env.arena.view(b_fc2_b)))
-            env.arena.handoff = (dx, dxb)
-        else:
-            dx = ops.layernorm_bwd(du, x, mean1, rstd1, n1w, dn1w, dn1b, dres=dx1)
+            dqkv, _, _ = ops.attn_bwd(qkv, ao, dao, lse, th, tw, Bp, heads, h, w, dT_out=dT, rel=rel,
+                                      table_grads=tables)
+        if need["qkv_b"]:
+            ops.colsum_bf16(dqkv, out=g["qkv_b"])
+        if need["qkv_w"]:
+            _wgrad(dqkv, u, out=g["qkv_w"])
+        dx = None
+        if need_du:
+            if ws > 0:
+                du = ops.gemm(dqkv, wqkv, trans_b=True, kind=EPI_F32)
+                du = ops.window_unpartition(du, Bp, h, w, ws)   # gradients at padded tokens are dropped
+            else:
+                du = ops.gemm(dqkv, wqkv, trans_b=True, kind=EPI_BF16)
+            # the block below consumes dx only through bf16(its DropPath scale * dx): emit that - and the fc2 bias
+            # gradient it implies, into its arena slot, unless that bias is frozen - in the same pass (with no arena
+            # and a trainable bias, the block below makes its own pass)
+            below = env.below if (env is not None and need_dx) else None
+            if below is not None and below[0].requires_grad and not act:
+                below = None
+            if below is not None:
+                b_fc2_b, b_drop_m, b_N = below
+                dx, dxb = ops.layernorm_bwd(du, x, mean1, rstd1, n1w, g["n1w"], g["n1b"], dres=dx1,
+                                            cast=(b_drop_m, b_N,
+                                                  env.arena.view(b_fc2_b) if b_fc2_b.requires_grad else None))
+                link.handoff = (dx, dxb)
+            else:
+                dx = ops.layernorm_bwd(du, x, mean1, rstd1, n1w, g["n1w"], g["n1b"], dres=dx1)
         if act:
             env.arena.stage_done(env.name)
-        return (dx, None, None, dn1w, dn1b, dTh, dTw, dqkv_w, dqkv_b, dproj_w, dproj_b, dn2w, dn2b, dfc1_w, dfc1_b,
-                dfc2_w, dfc2_b, None, None)
+        return (dx if need_dx else None, None, None, *[g[r] if need[r] else None for r in BLOCK_ROLES], None, None)
 
 
 class MergeFn(torch.autograd.Function):
@@ -311,7 +373,10 @@ class MergeFn(torch.autograd.Function):
 
 
 class DecoderFn(torch.autograd.Function):
-    """(4 tap activations) -> (loss[1], patchified prediction [B, N, p*p*3])."""
+    """(4 tap activations) -> (loss[1], patchified prediction [B, N, p*p*3]).  The loss's gradient with respect to
+    tgts (-dpred, from the fused head backward) is returned when tgts requires grad; autograd adds it to the encoder's.
+    Parameter gradients are computed only for parameters that require grad; `cat` / `g` (the operands of the
+    decoder-embed and 3x3 weight gradients) are saved only if those weights require grad."""
 
     @staticmethod
     def forward(ctx, t0, t1, t2, t3, norm_w, norm_b, dec_w, dec_b, c3_w, c3_b, ln_w, ln_b, c1_w, c1_b, tgts, mask_u8,
@@ -337,8 +402,9 @@ class DecoderFn(torch.autograd.Function):
         st = ops.loss_prep(tgts, mask_u8, valid, p)
         c1, patch, num = ops.decoder_head_fwd(g, wf, hp, tgts, mask_u8, valid, p, loss_kind)
         loss, coef = ops.loss_finalize(st, num, seggpt)
-        ctx.save_for_backward(t0, t1, t2, t3, norm_w, cat, wdec, g, wd, hp, c1, tgts, mask_u8, valid, coef,
-                              *[s for pair in stats for s in pair])
+        need = ctx.needs_input_grad
+        ctx.save_for_backward(t0, t1, t2, t3, norm_w, cat if need[6] else None, wdec, g if need[8] else None, wd, hp,
+                              c1, tgts, mask_u8, valid, coef, *[s for pair in stats for s in pair])
         ctx.meta = meta
         ctx.shapes = (c3_w.shape, c1_w.shape)
         ctx.mark_non_differentiable(patch)
@@ -353,33 +419,60 @@ class DecoderFn(torch.autograd.Function):
         B, h, w, p, eps, loss_kind, seggpt = ctx.meta
         M, C = t[0].shape
         dev = c1.device
+        need = ctx.needs_input_grad
         env = ctx.env
         act = env is not None and env.begin()
         G = (lambda k: env.grad(True, k)) if act else (lambda k: None)
         gscale = dloss.reshape(1).to(torch.float32).contiguous()
-        dc1, dhp = ops.decoder_head_bwd(c1, tgts, mask_u8, valid, coef, gscale, hp, p, loss_kind)
-        dc3_b = ops.colsum_bf16(dc1.view(-1, 64), out=G("c3_b"))
-        dc3_w = ops.conv3x3_wgrad(g, dc1, out=G("c3_w"))
-        dD = ops.conv3x3_dgrad_unshuffle(dc1, wd, p)          # [M, p*p*64] bf16, token-major
-        ddec_b = ops.colsum_bf16(dD, out=G("dec_b"))
-        ddec_w = _wgrad(dD, cat, out=G("dec_w"))
-        dcat = ops.gemm(dD, wdec, trans_b=True, kind=EPI_BF16)  # [M, 4C] bf16, read by the 4 LayerNorm backwards
-        dnw = G("norm_w") if act else torch.zeros(C, dtype=torch.float32, device=dev)
-        dnb = G("norm_b") if act else torch.zeros(C, dtype=torch.float32, device=dev)
-        dts = []
-        for k in range(4):
-            dts.append(ops.layernorm_bwd(dcat[:, k * C:(k + 1) * C], t[k], stats[2 * k], stats[2 * k + 1], norm_w,
-                                         dnw, dnb))
+        head = any(need[10:14])
+        dtg = None
+        if need[14]:
+            dc1, dhp, dtg = ops.decoder_head_bwd_dtgt(c1, tgts, mask_u8, valid, coef, gscale, hp, p, loss_kind,
+                                                      params=head)
+        else:
+            dc1, dhp = ops.decoder_head_bwd(c1, tgts, mask_u8, valid, coef, gscale, hp, p, loss_kind, params=head)
+        dc3_b = ops.colsum_bf16(dc1.view(-1, 64), out=G("c3_b")) if need[9] else None
+        dc3_w = ops.conv3x3_wgrad(g, dc1, out=G("c3_w")) if need[8] else None
+        ddec_w = ddec_b = dnw = dnb = None
+        dts = [None] * 4
+        if any(need[0:8]):
+            dD = ops.conv3x3_dgrad_unshuffle(dc1, wd, p)          # [M, p*p*64] bf16, token-major
+            ddec_b = ops.colsum_bf16(dD, out=G("dec_b")) if need[7] else None
+            ddec_w = _wgrad(dD, cat, out=G("dec_w")) if need[6] else None
+            if any(need[0:6]):
+                dcat = ops.gemm(dD, wdec, trans_b=True, kind=EPI_BF16)  # [M, 4C] bf16, read by the 4 LN backwards
+                if need[4]:
+                    dnw = G("norm_w") if act else torch.zeros(C, dtype=torch.float32, device=dev)
+                if need[5]:
+                    dnb = G("norm_b") if act else torch.zeros(C, dtype=torch.float32, device=dev)
+                for k in range(4):
+                    dts[k] = ops.layernorm_bwd(dcat[:, k * C:(k + 1) * C], t[k], stats[2 * k], stats[2 * k + 1],
+                                               norm_w, dnw, dnb)
         c3shape, c1shape = ctx.shapes
+        dlw = dlb = dc1w = dc1b = None
         if act:
-            dlw, dlb, dc1w, dc1b = G("ln_w"), G("ln_b"), G("c1_w"), G("c1_b")
-            dlw.copy_(dhp[64:128])
-            dlb.copy_(dhp[128:192])
-            dc1w.view(-1).copy_(dhp[192:384])
-            dc1b.copy_(dhp[384:387])
+            if need[10]:
+                dlw = G("ln_w")
+                dlw.copy_(dhp[64:128])
+            if need[11]:
+                dlb = G("ln_b")
+                dlb.copy_(dhp[128:192])
+            if need[12]:
+                dc1w = G("c1_w")
+                dc1w.view(-1).copy_(dhp[192:384])
+            if need[13]:
+                dc1b = G("c1_b")
+                dc1b.copy_(dhp[384:387])
             env.arena.stage_done(env.name)
         else:
-            dlw, dlb = dhp[64:128].clone(), dhp[128:192].clone()
-            dc1w, dc1b = dhp[192:384].reshape(c1shape).clone(), dhp[384:387].clone()
-        return (dts[0], dts[1], dts[2], dts[3], dnw, dnb, ddec_w, ddec_b, dc3_w, dc3_b, dlw, dlb, dc1w, dc1b, None,
-                None, None, None, None)
+            if need[10]:
+                dlw = dhp[64:128].clone()
+            if need[11]:
+                dlb = dhp[128:192].clone()
+            if need[12]:
+                dc1w = dhp[192:384].reshape(c1shape).clone()
+            if need[13]:
+                dc1b = dhp[384:387].clone()
+        return (dts[0] if need[0] else None, dts[1] if need[1] else None, dts[2] if need[2] else None,
+                dts[3] if need[3] else None, dnw, dnb, ddec_w, ddec_b, dc3_w, dc3_b, dlw, dlb, dc1w, dc1b, dtg, None,
+                None, None, None)

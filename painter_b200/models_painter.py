@@ -256,8 +256,10 @@ class Painter(nn.Module):
         h, w = H // p, W // p
         N, C = h * w, self.embed_dim
         dev = imgs.device
-        imgs = imgs.detach().float().contiguous()
-        tgts = tgts.detach().float().contiguous()
+        # imgs and tgts are differentiable inputs, as in the reference (prompt tuning learns them with every weight
+        # frozen); valid and bool_masked_pos are loss weights and a mask, not differentiable
+        imgs = imgs.float().contiguous()
+        tgts = tgts.float().contiguous()
         valid = valid.detach().float().contiguous()
         if valid.shape != tgts.shape:
             valid = valid.expand_as(tgts).contiguous()
@@ -271,11 +273,17 @@ class Painter(nn.Module):
             if self.training and any(b.drop_prob > 0 for b in self.blocks):
                 raise NotImplementedError("painter_b200: the fp32-accurate mode is an inference mode (call .eval())")
             from . import accurate
-            return accurate.forward(self, imgs, tgts, mask_u8, valid, self._type_emb(B, seg_type, dev),
-                                    merge_between_batch)
+            return accurate.forward(self, imgs.detach(), tgts.detach(), mask_u8, valid,
+                                    self._type_emb(B, seg_type, dev), merge_between_batch)
         pe = self.patch_embed.proj
-        # gradient arena + per-step token (engine.StageEnv): only when this forward can be followed by a backward
-        arena = get_arena(self) if torch.is_grad_enabled() else None
+        # gradient arena + per-step token (engine.StageEnv): only when this forward can be followed by a backward that
+        # produces parameter gradients.  A fully frozen module (e.g. for prompt tuning) has none, and drops the arena
+        # of an earlier training phase.
+        trainable = any(q.requires_grad for q in self.parameters())
+        if not trainable:
+            self.__dict__.pop("_pk_arena", None)
+        arena = get_arena(self) if torch.is_grad_enabled() and trainable else None
+        link = engine.StepLink() if torch.is_grad_enabled() else None   # the block backwards' hand-off
         token = object()
         emb_prm = {"w": pe.weight, "b": pe.bias, "mt": self.mask_token, "sx": self.segment_token_x,
                    "sy": self.segment_token_y, "pe": self.pos_embed}
@@ -300,13 +308,13 @@ class Painter(nn.Module):
             rel_w = engine.resize_rel_table(a.rel_pos_w, ws if ws > 0 else w)
             prm = blk.params()
             env = None
-            if arena is not None:
+            if link is not None:
                 # hand-off: block i's dx is consumed only by block i-1's MLP branch (as bf16(DropPath scale * dx))
                 # unless block i-1's output also feeds the early merge or a decoder tap
                 below = None
                 if i > 0 and (i - 1) != merge_idx and (i - 1) not in (5, 11, 17, 23) and ens_g == 0:
                     below = (self.blocks[i - 1].mlp.fc2.bias, drops[i - 1][1], N)
-                env = StageEnv(arena, token, f"block{i}", blk.roles(), below)
+                env = StageEnv(arena, token, f"block{i}", blk.roles(), below, link)
             z = BlockFn.apply(z, da, dm, prm[0], prm[1], rel_h, rel_w, *prm[4:],
                               (Bp, h, w, self.num_heads, blk.norm1.eps, ens_g, ens_p, ws), env)
             if i == merge_idx:

@@ -142,16 +142,20 @@ def attn_fwd_split3(qkv, th, tw, B, heads, h, w):
     return out
 
 
-def attn_bwd(qkv, out, dout, lse, th, tw, B, heads, h, w, L_h=None, L_w=None, dT_out=None, rel=None):
+def attn_bwd(qkv, out, dout, lse, th, tw, B, heads, h, w, L_h=None, L_w=None, dT_out=None, rel=None,
+             table_grads=True):
     """Fused attention backward.  Returns (dqkv bf16 [B*N, 3C], dTh fp32 [2h-1, 64], dTw fp32 [2w-1, 64]).
     rel: the (relh, relw) buffers of `attn_fwd(..., save_rel=True)` on the same operands (the dQ kernel then loads its
-    bias rows instead of recomputing them)."""
+    bias rows instead of recomputing them).  table_grads=False (frozen tables): dTh = dTw = None, the table-gradient
+    work is skipped and dqkv is bit-identical."""
     N, C = h * w, heads * 64
     _req(dout, torch.bfloat16, "dout")
     assert dout.is_contiguous() and out.is_contiguous() and qkv.is_contiguous()
     dev = qkv.device
     dqkv = torch.empty_like(qkv)
-    if dT_out is not None:       # caller-provided, zero-initialised (or running) fp32 accumulators
+    if not table_grads:
+        dTh = dTw = None
+    elif dT_out is not None:       # caller-provided, zero-initialised (or running) fp32 accumulators
         dTh, dTw = dT_out
         assert tuple(dTh.shape) == (2 * h - 1, 64) and tuple(dTw.shape) == (2 * w - 1, 64)
         assert dTh.is_contiguous() and dTw.is_contiguous() and dTh.dtype == torch.float32
@@ -162,7 +166,8 @@ def attn_bwd(qkv, out, dout, lse, th, tw, B, heads, h, w, L_h=None, L_w=None, dT
     Np = (N + 127) // 128 * 128     # the bias-row scratch is laid out in whole 128-query tiles
     L = lib()
     L.pk_attn_bwd_ws_floats.restype = ctypes.c_longlong
-    dt_ws = torch.empty((int(L.pk_attn_bwd_ws_floats(B, heads, h, w)),), dtype=torch.float32, device=dev)
+    dt_ws = (torch.empty((int(L.pk_attn_bwd_ws_floats(B, heads, h, w)),), dtype=torch.float32, device=dev)
+             if table_grads else None)
     if rel is not None:
         relh_g, relw_g = rel
         assert relh_g.numel() == B * heads * Np * h and relw_g.numel() == B * heads * Np * w
@@ -202,7 +207,8 @@ def layernorm_fwd(x, gamma, beta, eps, out=None, out_dtype=torch.bfloat16, want_
 def layernorm_bwd(dy, x, mean, rstd, gamma, dgamma, dbeta, dres=None, cast=None):
     """Returns dx fp32 [M, C] (+ dres); accumulates into dgamma / dbeta (fp32, caller-initialised).
     cast = (rowscale or None, rows_per_group, colsum_out[C]): also returns bf16(rowscale * dx) and adds its column
-    sums to colsum_out (the fused form of `scale_cast_colsum(layernorm_bwd(...))`)."""
+    sums to colsum_out (the fused form of `scale_cast_colsum(layernorm_bwd(...))`).
+    dgamma = dbeta = None (frozen LayerNorm) / colsum_out = None: that reduction is skipped; dx is unchanged."""
     if dy.dtype != torch.bfloat16:
         _req(dy, torch.float32, "dy")
     dyb = int(dy.dtype == torch.bfloat16)
@@ -214,7 +220,8 @@ def layernorm_bwd(dy, x, mean, rstd, gamma, dgamma, dbeta, dres=None, cast=None)
         assert dres.is_contiguous()
     L = lib()
     L.pk_layernorm_bwd_ws_floats.restype = ctypes.c_longlong
-    ws = torch.empty((int(L.pk_layernorm_bwd_ws_floats(M, C)),), dtype=torch.float32, device=x.device)
+    sums = dgamma is not None or dbeta is not None or (cast is not None and cast[2] is not None)
+    ws = torch.empty((int(L.pk_layernorm_bwd_ws_floats(M, C)),), dtype=torch.float32, device=x.device) if sums else None
     if cast is not None:
         rowscale, rpg, cs = cast
         dxb = torch.empty((M, C), dtype=torch.bfloat16, device=x.device)
@@ -239,6 +246,21 @@ def im2col_patch(imgs, tgts, p):
     return out
 
 
+def col2im_patch(dcols_x, dcols_y, B, Cin, H, W, p):
+    """Input gradient of `im2col_patch`: the patch-embed dgrad of the x rows / y rows, fp32 [B*(H/p)*(W/p), Cin*p*p]
+    each (None: that half is not wanted) -> (dimgs, dtgts) fp32 NCHW, None where not wanted."""
+    out = []
+    for d in (dcols_x, dcols_y):
+        if d is not None:
+            _req(d, torch.float32, "dcols")
+            assert d.is_contiguous() and tuple(d.shape) == (B * (H // p) * (W // p), Cin * p * p)
+        out.append(torch.empty((B, Cin, H, W), dtype=torch.float32, device=d.device) if d is not None else None)
+    dimgs, dtgts = out
+    check(lib().pk_col2im_patch(_ptr(dcols_x), _ptr(dcols_y), _ptr(dimgs), _ptr(dtgts), B, Cin, H, W, p, _stream()),
+          "pk_col2im_patch")
+    return dimgs, dtgts
+
+
 def assemble_tokens(E, mask_u8, mask_token, seg_x, seg_y, pos, type_emb, B, N, C):
     out = torch.empty_like(E)
     check(lib().pk_assemble_tokens(_ptr(E), _ptr(mask_u8), mask_u8.shape[0], _ptr(mask_token), _ptr(seg_x),
@@ -247,12 +269,15 @@ def assemble_tokens(E, mask_u8, mask_token, seg_x, seg_y, pos, type_emb, B, N, C
     return out
 
 
-def assemble_tokens_bwd(dZ, mask_u8, B, N, C, token_grads=None):
-    """token_grads: optional (dseg_x, dseg_y, dmask_token) zero-initialised fp32 [C] accumulators (arena views)."""
+def assemble_tokens_bwd(dZ, mask_u8, B, N, C, token_grads=None, want_tokens=True, want_pos=True):
+    """token_grads: optional (dseg_x, dseg_y, dmask_token) zero-initialised fp32 [C] accumulators (arena views).
+    want_tokens=False / want_pos=False (frozen parameters): those gradients are skipped and returned as None."""
     dev = dZ.device
     dE = torch.empty((2 * B * N, C), dtype=torch.bfloat16, device=dev)
-    dpos = torch.empty((N, C), dtype=torch.float32, device=dev)
-    if token_grads is None:
+    dpos = torch.empty((N, C), dtype=torch.float32, device=dev) if want_pos else None
+    if not want_tokens:
+        token_grads = (None, None, None)
+    elif token_grads is None:
         small = torch.zeros((3, C), dtype=torch.float32, device=dev)
         token_grads = (small[0], small[1], small[2])
     sx, sy, mt = token_grads
@@ -371,14 +396,28 @@ def loss_finalize(stats, num, seggpt):
     return loss, coef
 
 
-def decoder_head_bwd(c1, tgts, mask_u8, valid, coef, gscale, head_params, p, loss_kind):
+def decoder_head_bwd(c1, tgts, mask_u8, valid, coef, gscale, head_params, p, loss_kind, params=True):
+    """Returns (dc1 bf16 NHWC, dhp fp32 [392]); params=False (frozen head): no parameter reductions, dhp is None."""
     B, H, W, _ = c1.shape
     dc1 = torch.empty_like(c1)
-    dhp = torch.zeros((392,), dtype=torch.float32, device=c1.device)
+    dhp = torch.zeros((392,), dtype=torch.float32, device=c1.device) if params else None
     check(lib().pk_decoder_head_bwd(_ptr(c1), _ptr(tgts), _ptr(mask_u8), mask_u8.shape[0], _ptr(valid), _ptr(coef),
                                     _ptr(gscale), _ptr(head_params), _ptr(dc1), _ptr(dhp), B, H, W, p, loss_kind,
                                     _stream()), "pk_decoder_head_bwd")
     return dc1, dhp
+
+
+def decoder_head_bwd_dtgt(c1, tgts, mask_u8, valid, coef, gscale, head_params, p, loss_kind, params=True):
+    """decoder_head_bwd that also returns the loss's gradient with respect to the targets, dtgts fp32 NCHW = -dpred
+    (not including the targets' path through the encoder): (dc1, dhp or None, dtgts)."""
+    B, H, W, _ = c1.shape
+    dc1 = torch.empty_like(c1)
+    dhp = torch.zeros((392,), dtype=torch.float32, device=c1.device) if params else None
+    dt = torch.empty(tgts.shape, dtype=torch.float32, device=c1.device)
+    check(lib().pk_decoder_head_bwd_dtgt(_ptr(c1), _ptr(tgts), _ptr(mask_u8), mask_u8.shape[0], _ptr(valid),
+                                         _ptr(coef), _ptr(gscale), _ptr(head_params), _ptr(dc1), _ptr(dhp), _ptr(dt),
+                                         B, H, W, p, loss_kind, _stream()), "pk_decoder_head_bwd_dtgt")
+    return dc1, dhp, dt
 
 
 def conv3x3_dgrad_unshuffle(dc1, wd, p):
