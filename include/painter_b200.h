@@ -118,6 +118,14 @@ int pk_assemble_tokens(const float* E, const uint8_t* mask, int maskB, const flo
                        float* out, int B, int N, int C, void* stream);
 int pk_assemble_tokens_bwd(const float* dZ, const uint8_t* mask, int maskB, void* dE_bf16, float* dpos,
                            float* dseg_x, float* dseg_y, float* dmask_token, int B, int N, int C, void* stream);
+/* The same backward with the SegGPT type-token gradients (models_seggpt.py:415-420): seg_type fp32 [B] on the device;
+ * dtype_cls / dtype_ins [C] (atomically accumulated, caller zero-initialises) receive sum_n (dZ[b, n] + dZ[B + b, n])
+ * over the samples with seg_type[b] == 0 / == 1; other values contribute to neither.  dtype_cls = dtype_ins = NULL
+ * (both) skips that reduction and seg_type is then not read.  pk_assemble_tokens_bwd is this call with all three
+ * NULL; dE, dpos and the other token gradients do not depend on them.                                           */
+int pk_assemble_tokens_bwd_typed(const float* dZ, const uint8_t* mask, int maskB, void* dE_bf16, float* dpos,
+                                 float* dseg_x, float* dseg_y, float* dmask_token, const float* seg_type,
+                                 float* dtype_cls, float* dtype_ins, int B, int N, int C, void* stream);
 
 /* get_abs_pos (util/vitdet_utils.py:141-157): F.interpolate(bicubic, align_corners=False), NHWC [sh,sw,C] ->
  * [h,w,C]; bwd scatters atomically into a zero-initialised [sh,sw,C].                                      */

@@ -308,21 +308,34 @@ assemble_kernel(const float* __restrict__ E, const uint8_t* __restrict__ mask, i
   }
 }
 
-// backward of the assembly: dE (bf16, y rows gated by 1-m), dpos[N,C], dseg_x, dseg_y, dmask_token
+// backward of the assembly: dE (bf16, y rows gated by 1-m), dpos[N,C], dseg_x, dseg_y, dmask_token and the SegGPT
+// type tokens (models_seggpt.py:415-420: sample b's x and y rows feed type_token_cls when seg_type[b] == 0,
+// type_token_ins when it is 1, neither otherwise; seg_type is compared as fp32, like the forward's mask arithmetic)
 // block = (C/4, TY) threads, one token per threadIdx.y
 __global__ void assemble_bwd_kernel(const float* __restrict__ dZ, const uint8_t* __restrict__ mask,
                                     int maskB, __nv_bfloat16* __restrict__ dE, float* __restrict__ dpos,
                                     float* __restrict__ dseg_x, float* __restrict__ dseg_y,
-                                    float* __restrict__ dmask_token, int B, int N, int C) {
-  extern __shared__ float4 sred[];  // [3][TY][C/4]
+                                    float* __restrict__ dmask_token, const float* __restrict__ seg_type,
+                                    float* __restrict__ dtype_cls, float* __restrict__ dtype_ins, int B, int N,
+                                    int C) {
+  extern __shared__ float4 sred[];  // [3 or 5][TY][C/4]
   const int c4n = C / 4;
   const int c4 = threadIdx.x;
   const int n = blockIdx.x * blockDim.y + threadIdx.y;
-  float4 sx = make_float4(0, 0, 0, 0), sy = sx, sm = sx;
+  const bool tok = dseg_x != nullptr, typ = dtype_cls != nullptr;
+  float4 sx = make_float4(0, 0, 0, 0), sy = sx, sm = sx, tc = sx, ti = sx;
   if (n < N) {
     for (int img = 0; img < 2 * B; ++img) {
       const size_t off = (static_cast<size_t>(img) * N + n) * c4n + c4;
       float4 d = reinterpret_cast<const float4*>(dZ)[off];
+      if (typ) {
+        const float st = __ldg(seg_type + (img < B ? img : img - B));
+        if (st == 0.f) {
+          tc.x += d.x; tc.y += d.y; tc.z += d.z; tc.w += d.w;
+        } else if (st == 1.f) {
+          ti.x += d.x; ti.y += d.y; ti.z += d.z; ti.w += d.w;
+        }
+      }
       if (img < B) {
         sx.x += d.x; sx.y += d.y; sx.z += d.z; sx.w += d.w;
       } else {
@@ -341,20 +354,29 @@ __global__ void assemble_bwd_kernel(const float* __restrict__ dZ, const uint8_t*
       reinterpret_cast<float4*>(dpos)[static_cast<size_t>(n) * c4n + c4] =
           make_float4(sx.x + sy.x, sx.y + sy.y, sx.z + sy.z, sx.w + sy.w);
   }
-  if (dseg_x == nullptr) return;   // frozen tokens: no reduction (the host passes all three or none)
+  if (!tok && !typ) return;   // frozen tokens: no reduction
+  // slots 0..2: dseg_x, dseg_y, dmask_token (all three or none); slots 3..4: dtype_cls, dtype_ins (both or none)
   const int TY = blockDim.y;
-  sred[(0 * TY + threadIdx.y) * c4n + c4] = sx;
-  sred[(1 * TY + threadIdx.y) * c4n + c4] = sy;
-  sred[(2 * TY + threadIdx.y) * c4n + c4] = sm;
+  const size_t slot = static_cast<size_t>(TY) * c4n;
+  float4* mine = sred + threadIdx.y * c4n + c4;
+  if (tok) {
+    mine[0] = sx;
+    mine[slot] = sy;
+    mine[2 * slot] = sm;
+  }
+  if (typ) {
+    mine[3 * slot] = tc;
+    mine[4 * slot] = ti;
+  }
   __syncthreads();
-  if (threadIdx.y < 3) {
-    const int which = threadIdx.y;
+  for (int which = tok ? threadIdx.y : threadIdx.y + 3; which < (typ ? 5 : 3); which += TY) {
     float4 s = make_float4(0, 0, 0, 0);
     for (int t = 0; t < TY; ++t) {
-      const float4 v = sred[(which * TY + t) * c4n + c4];
+      const float4 v = sred[which * slot + t * c4n + c4];
       s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
     }
-    float* dst = (which == 0 ? dseg_x : (which == 1 ? dseg_y : dmask_token)) + c4 * 4;
+    float* dst = (which == 0 ? dseg_x : which == 1 ? dseg_y : which == 2 ? dmask_token :
+                  which == 3 ? dtype_cls : dtype_ins) + c4 * 4;
     atomicAdd(dst + 0, s.x); atomicAdd(dst + 1, s.y); atomicAdd(dst + 2, s.z); atomicAdd(dst + 3, s.w);
   }
 }
@@ -691,30 +713,43 @@ extern "C" int pk_assemble_tokens(const float* E, const uint8_t* mask, int maskB
   return 0;
 }
 
-extern "C" int pk_assemble_tokens_bwd(const float* dZ, const uint8_t* mask, int maskB, void* dE_bf16,
-                                      float* dpos, float* dseg_x, float* dseg_y, float* dmask_token, int B,
-                                      int N, int C, void* stream) {
+extern "C" int pk_assemble_tokens_bwd_typed(const float* dZ, const uint8_t* mask, int maskB, void* dE_bf16,
+                                            float* dpos, float* dseg_x, float* dseg_y, float* dmask_token,
+                                            const float* seg_type, float* dtype_cls, float* dtype_ins, int B, int N,
+                                            int C, void* stream) {
   // dpos = NULL: the position gradient is not needed; dseg_x = dseg_y = dmask_token = NULL: the token gradients are
-  // not needed (all three or none).  dE is unchanged either way.
+  // not needed (all three or none); dtype_cls = dtype_ins = NULL: no type-token gradients (both or none, and then
+  // seg_type is not read).  dE is unchanged either way.
   PK_CHECK(dZ && mask && dE_bf16, "pk_assemble_tokens_bwd: null pointer");
   PK_CHECK((dseg_x != nullptr) == (dseg_y != nullptr) && (dseg_x != nullptr) == (dmask_token != nullptr),
            "pk_assemble_tokens_bwd: dseg_x, dseg_y and dmask_token must all be given or all be NULL");
+  PK_CHECK((dtype_cls != nullptr) == (dtype_ins != nullptr) && (dtype_cls == nullptr || seg_type != nullptr),
+           "pk_assemble_tokens_bwd: dtype_cls and dtype_ins must both be given (with seg_type) or both be NULL");
   PK_CHECK(C % 4 == 0 && C / 4 <= 256, "pk_assemble_tokens_bwd: C=%d unsupported", C);
   const int tx = C / 4;
   int ty = 1024 / tx;
   if (ty > 8) ty = 8;
   if (ty < 3) ty = 3;
   PK_CHECK(tx * ty <= 1024, "pk_assemble_tokens_bwd: C too large");
-  const size_t smem = static_cast<size_t>(3) * ty * tx * sizeof(float4);
+  const int slots = dtype_cls ? 5 : 3;
+  const size_t smem = static_cast<size_t>(slots) * ty * tx * sizeof(float4);
   static bool attr = false;
   if (!attr) {
-    cudaFuncSetAttribute(assemble_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 3 * 8 * 256 * 16);
+    cudaFuncSetAttribute(assemble_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 5 * 1024 * 16);
     attr = true;
   }
   assemble_bwd_kernel<<<(N + ty - 1) / ty, dim3(tx, ty), smem, static_cast<cudaStream_t>(stream)>>>(
-      dZ, mask, maskB, static_cast<__nv_bfloat16*>(dE_bf16), dpos, dseg_x, dseg_y, dmask_token, B, N, C);
+      dZ, mask, maskB, static_cast<__nv_bfloat16*>(dE_bf16), dpos, dseg_x, dseg_y, dmask_token, seg_type, dtype_cls,
+      dtype_ins, B, N, C);
   PK_LAUNCH_CHECK("pk_assemble_tokens_bwd");
   return 0;
+}
+
+extern "C" int pk_assemble_tokens_bwd(const float* dZ, const uint8_t* mask, int maskB, void* dE_bf16,
+                                      float* dpos, float* dseg_x, float* dseg_y, float* dmask_token, int B,
+                                      int N, int C, void* stream) {
+  return pk_assemble_tokens_bwd_typed(dZ, mask, maskB, dE_bf16, dpos, dseg_x, dseg_y, dmask_token, nullptr, nullptr,
+                                      nullptr, B, N, C, stream);
 }
 
 extern "C" int pk_bicubic_fwd(const float* src, float* dst, int sh, int sw, int h, int w, int C, void* stream) {

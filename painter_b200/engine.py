@@ -109,13 +109,24 @@ def resize_rel_table(table, size):
     return F.interpolate(table.t().unsqueeze(0), size=L, mode="linear")[0].t().contiguous()
 
 
+def type_embedding(seg_type, type_cls, type_ins):
+    """SegGPT's per-sample type embedding [B, C] fp32 (models_seggpt.py:415-417): type_token_cls where seg_type is 0,
+    type_token_ins where it is 1, zero otherwise.  Mask arithmetic instead of boolean indexing: no host
+    synchronisation, so the step stays CUDA-graph capturable.  seg_type: fp32 [B, 1] on the device."""
+    C = type_cls.shape[-1]
+    return ((seg_type == 0).to(torch.float32) * type_cls.reshape(1, C).float() +
+            (seg_type == 1).to(torch.float32) * type_ins.reshape(1, C).float()).contiguous()
+
+
 class EmbedFn(torch.autograd.Function):
     """imgs, tgts fp32 NCHW -> tokens [2B*N, C].  Gradients flow to imgs / tgts (prompt tuning, saliency) through the
     patch-embed dgrad and pk_col2im_patch; every parameter gradient is computed only if that parameter requires grad
-    (the weight gradient's operand `cols` is not even saved when the weight is frozen)."""
+    (the weight gradient's operand `cols` is not even saved when the weight is frozen).  SegGPT passes seg_type (fp32
+    [B, 1] on the device) and its two type tokens; Painter passes None for all three."""
 
     @staticmethod
-    def forward(ctx, imgs, tgts, mask_u8, type_emb, Wp, bp, mask_token, seg_x, seg_y, pos_embed, p, has_cls, env):
+    def forward(ctx, imgs, tgts, mask_u8, seg_type, Wp, bp, mask_token, seg_x, seg_y, pos_embed, type_cls, type_ins,
+                p, has_cls, env):
         B, Cin, H, W = imgs.shape
         h, w = H // p, W // p
         N, C = h * w, Wp.shape[0]
@@ -127,30 +138,35 @@ class EmbedFn(torch.autograd.Function):
         assert s * s == pe.shape[0]
         pe = pe.contiguous()
         pos = pe if (s == h and s == w) else ops.bicubic_fwd(pe.view(s, s, C), h, w).view(N, C)
+        type_emb = None if seg_type is None else type_embedding(seg_type, type_cls, type_ins)
         z = ops.assemble_tokens(E, mask_u8, mask_token.reshape(C).contiguous(), seg_x.reshape(C).contiguous(),
                                 seg_y.reshape(C).contiguous(), pos, type_emb, B, N, C)
         need = ctx.needs_input_grad
-        ctx.save_for_backward(cols if need[4] else None, mask_u8, wp if (need[0] or need[1]) else None)
-        ctx.meta = (B, N, C, h, w, s, has_cls, Wp.shape, pos_embed.shape, mask_token.shape, type_emb is not None,
+        need_type = seg_type is not None and (need[10] or need[11])
+        ctx.save_for_backward(cols if need[4] else None, mask_u8, wp if (need[0] or need[1]) else None,
+                              seg_type.reshape(B).contiguous() if need_type else None)
+        ctx.meta = (B, N, C, h, w, s, has_cls, Wp.shape, pos_embed.shape, mask_token.shape, need_type,
                     (Cin, H, W, p))
         ctx.env = env
         return z
 
     @staticmethod
     def backward(ctx, dz):
-        cols, mask_u8, wp = ctx.saved_tensors
-        B, N, C, h, w, s, has_cls, wshape, pshape, tshape, has_type, (Cin, H, W, p) = ctx.meta
+        cols, mask_u8, wp, seg_type = ctx.saved_tensors
+        B, N, C, h, w, s, has_cls, wshape, pshape, tshape, need_type, (Cin, H, W, p) = ctx.meta
         need = ctx.needs_input_grad
-        if has_type and need[3]:
-            raise NotImplementedError("painter_b200: gradients of the SegGPT type tokens are not implemented "
-                                      "(SegGPT is an inference path, seggpt_engine.py:26)")
         env = ctx.env
         act = env is not None and env.begin()
         dz = dz.contiguous()
         need_tok = need[6] or need[7] or need[8]
         tok = tuple(env.grad(True, k).view(C) for k in ("sx", "sy", "mt")) if act and need_tok else None
+        typ = None
+        if need_type:   # both type tokens are reduced in one pass, even when only one of them requires grad
+            dtt = tuple(env.grad(True, k).view(C) for k in ("tc", "ti")) if act else \
+                torch.zeros((2, C), dtype=torch.float32, device=dz.device).unbind(0)
+            typ = (seg_type, *dtt)
         dE, dpos, dsx, dsy, dmt = ops.assemble_tokens_bwd(dz, mask_u8, B, N, C, token_grads=tok, want_tokens=need_tok,
-                                                          want_pos=need[9])
+                                                          want_pos=need[9], type_grads=typ)
         dW = _wgrad(dE, cols, out=env.grad(True, "w").view(wshape[0], -1) if act else None).view(wshape) \
             if need[4] else None
         db = ops.colsum_bf16(dE, out=env.grad(True, "b") if act else None) if need[5] else None
@@ -174,10 +190,12 @@ class EmbedFn(torch.autograd.Function):
             env.arena.stage_done(env.name)
             env.arena.end_backward()
             return (dimgs, dtgts, None, None, dW, db, env.grad(True, "mt") if need[6] else None,
-                    env.grad(True, "sx") if need[7] else None, env.grad(True, "sy") if need[8] else None, dpe, None,
+                    env.grad(True, "sx") if need[7] else None, env.grad(True, "sy") if need[8] else None, dpe,
+                    env.grad(True, "tc") if need[10] else None, env.grad(True, "ti") if need[11] else None, None,
                     None, None)
         return (dimgs, dtgts, None, None, dW, db, dmt.view(tshape) if need[6] else None,
-                dsx.view(tshape) if need[7] else None, dsy.view(tshape) if need[8] else None, dpe, None, None, None)
+                dsx.view(tshape) if need[7] else None, dsy.view(tshape) if need[8] else None, dpe,
+                typ[1].view(tshape) if need[10] else None, typ[2].view(tshape) if need[11] else None, None, None, None)
 
 
 # BlockFn's parameter inputs (positions 3 .. 16 of its forward) in the order of models_painter.Block.ROLES

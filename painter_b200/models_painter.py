@@ -243,8 +243,13 @@ class Painter(nn.Module):
         """Per-block view of the step's DropPath scales (tests replace this to replay the reference's CPU draws)."""
         return self._step_drops.get(i, (None, None))
 
+    def _type_inputs(self, B, seg_type, device):
+        """(seg_type fp32 [B, 1] on the device, type_token_cls, type_token_ins) for SegGPT; Painter has no type tokens."""
+        return None, None, None
+
     def _type_emb(self, B, seg_type, device):
-        return None
+        st, cls, ins = self._type_inputs(B, seg_type, device)
+        return None if st is None else engine.type_embedding(st, cls.detach(), ins.detach())
 
     def _run(self, imgs, tgts, bool_masked_pos, valid, seg_type=None, merge_between_batch=-1):
         if not imgs.is_cuda:
@@ -287,8 +292,11 @@ class Painter(nn.Module):
         token = object()
         emb_prm = {"w": pe.weight, "b": pe.bias, "mt": self.mask_token, "sx": self.segment_token_x,
                    "sy": self.segment_token_y, "pe": self.pos_embed}
-        z = EmbedFn.apply(imgs, tgts, mask_u8, self._type_emb(B, seg_type, dev), pe.weight, pe.bias, self.mask_token,
-                          self.segment_token_x, self.segment_token_y, self.pos_embed, p, self.pretrain_use_cls_token,
+        st, type_cls, type_ins = self._type_inputs(B, seg_type, dev)
+        if st is not None:
+            emb_prm.update(tc=type_cls, ti=type_ins)
+        z = EmbedFn.apply(imgs, tgts, mask_u8, st, pe.weight, pe.bias, self.mask_token, self.segment_token_x,
+                          self.segment_token_y, self.pos_embed, type_cls, type_ins, p, self.pretrain_use_cls_token,
                           StageEnv(arena, token, "embed", emb_prm) if arena is not None else None)
         merge_idx = 2
         Bp = 2 * B

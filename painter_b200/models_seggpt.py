@@ -21,14 +21,11 @@ class SegGPT(Painter):
         torch.nn.init.normal_(self.type_token_cls, std=.02)
         torch.nn.init.normal_(self.type_token_ins, std=.02)
 
-    def _type_emb(self, B, seg_type, device):
-        # models_seggpt.py:415-417 - tiny [B, C] parameter select (mask arithmetic instead of boolean indexing: no
-        # host synchronisation, so the forward stays CUDA-graph capturable)
-        C = self.embed_dim
+    def _type_inputs(self, B, seg_type, device):
+        # models_seggpt.py:415-420: seg_type 0 selects type_token_cls, 1 type_token_ins, anything else neither; the
+        # tokens are autograd inputs of the embedding (engine.EmbedFn), which reduces their gradients on the device
         st = seg_type.reshape(B, 1).to(device=device, dtype=torch.float32)
-        te = (st == 0).to(torch.float32) * self.type_token_cls.reshape(1, C).float() + \
-             (st == 1).to(torch.float32) * self.type_token_ins.reshape(1, C).float()
-        return te.detach().contiguous()
+        return st, self.type_token_cls, self.type_token_ins
 
     def forward(self, imgs, tgts, bool_masked_pos=None, valid=None, seg_type=None, merge_between_batch=-1):
         if bool_masked_pos is None:

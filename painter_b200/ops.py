@@ -269,9 +269,11 @@ def assemble_tokens(E, mask_u8, mask_token, seg_x, seg_y, pos, type_emb, B, N, C
     return out
 
 
-def assemble_tokens_bwd(dZ, mask_u8, B, N, C, token_grads=None, want_tokens=True, want_pos=True):
+def assemble_tokens_bwd(dZ, mask_u8, B, N, C, token_grads=None, want_tokens=True, want_pos=True, type_grads=None):
     """token_grads: optional (dseg_x, dseg_y, dmask_token) zero-initialised fp32 [C] accumulators (arena views).
-    want_tokens=False / want_pos=False (frozen parameters): those gradients are skipped and returned as None."""
+    want_tokens=False / want_pos=False (frozen parameters): those gradients are skipped and returned as None.
+    type_grads: optional (seg_type fp32 [B], dtype_cls, dtype_ins) - SegGPT's type-token gradients are accumulated
+    into the two zero-initialised fp32 [C] buffers in the same pass."""
     dev = dZ.device
     dE = torch.empty((2 * B * N, C), dtype=torch.bfloat16, device=dev)
     dpos = torch.empty((N, C), dtype=torch.float32, device=dev) if want_pos else None
@@ -281,9 +283,14 @@ def assemble_tokens_bwd(dZ, mask_u8, B, N, C, token_grads=None, want_tokens=True
         small = torch.zeros((3, C), dtype=torch.float32, device=dev)
         token_grads = (small[0], small[1], small[2])
     sx, sy, mt = token_grads
-    check(lib().pk_assemble_tokens_bwd(_ptr(dZ), _ptr(mask_u8), mask_u8.shape[0], _ptr(dE), _ptr(dpos),
-                                       _ptr(sx), _ptr(sy), _ptr(mt), B, N, C, _stream()),
-          "pk_assemble_tokens_bwd")
+    st, tc, ti = type_grads if type_grads is not None else (None, None, None)
+    if st is not None:
+        _req(st, torch.float32, "seg_type")
+        assert st.is_contiguous() and st.numel() == B
+    check(lib().pk_assemble_tokens_bwd_typed(_ptr(dZ), _ptr(mask_u8), mask_u8.shape[0], _ptr(dE), _ptr(dpos),
+                                             _ptr(sx), _ptr(sy), _ptr(mt), _ptr(st), _ptr(tc), _ptr(ti), B, N, C,
+                                             _stream()),
+          "pk_assemble_tokens_bwd_typed")
     return dE, dpos, sx, sy, mt
 
 

@@ -91,6 +91,10 @@ class GraphedTrainStep:
             adjust_learning_rate(optimizer, ...)             # per-iteration schedules keep working (see below)
             loss = step(samples, targets, bool_masked_pos, valid)     # 0-dim device tensor (static buffer)
 
+    A SegGPT module takes its per-sample seg types as a fifth input, `step(samples, targets, bool_masked_pos, valid,
+    seg_type)` ([B, 1]: 0 semantic, 1 instance); they get a static buffer like the other inputs, so every replay
+    reads the current batch's types.
+
     What makes the step capture-safe: gradients live in the module's flat arena (static addresses, zeroed by the
     optimizer kernel), the bf16 operand copies are refreshed by the optimizer kernel, DropPath draws come from the
     graph-registered CUDA generator, and everything that changes from one iteration to the next - learning rates,
@@ -104,17 +108,19 @@ class GraphedTrainStep:
         if not isinstance(optimizer, FusedAdamW):
             raise TypeError("GraphedTrainStep needs painter_b200.optim.FusedAdamW")
         self.model, self.opt, self.warmup, self.dtype = model, optimizer, warmup, autocast_dtype
+        self.seggpt = getattr(model, "seggpt", False)
         self.entries = {}
 
     def _eager(self, si):
+        kw = {"seg_type": si[4]} if self.seggpt else {}
         with torch.autocast("cuda", dtype=self.dtype):
-            loss, _, _ = self.model(si[0], si[1], bool_masked_pos=si[2], valid=si[3])
+            loss, _, _ = self.model(si[0], si[1], bool_masked_pos=si[2], valid=si[3], **kw)
         loss.backward()
         return loss
 
-    def _capture(self, imgs, tgts, mask, valid):
+    def _capture(self, inputs):
         dev = next(self.model.parameters()).device
-        si = [t.detach().to(dev, copy=True) for t in (imgs, tgts, mask, valid)]
+        si = [t.detach().to(dev, copy=True) for t in inputs]
         params = [p for g in self.opt.param_groups for p in g["params"]]
         # snapshot everything the warm-up iterations change
         with torch.no_grad():
@@ -167,19 +173,21 @@ class GraphedTrainStep:
         torch.cuda.synchronize(dev)
         return si, g, out
 
-    def __call__(self, imgs, tgts, bool_masked_pos, valid):
+    def __call__(self, imgs, tgts, bool_masked_pos, valid, seg_type=None):
         # inputs may live on the device or in (pinned) host memory: they are copied into the graph's static buffers
-        key = (tuple(imgs.shape), imgs.dtype, tuple(bool_masked_pos.shape), bool_masked_pos.dtype, tuple(valid.shape))
+        if self.seggpt != (seg_type is not None):
+            raise ValueError("GraphedTrainStep: seg_type is required for a SegGPT module and not accepted otherwise")
+        inputs = (imgs, tgts, bool_masked_pos, valid) + ((seg_type,) if seg_type is not None else ())
+        key = (tuple(imgs.shape), imgs.dtype, tuple(bool_masked_pos.shape), bool_masked_pos.dtype, tuple(valid.shape),
+               None if seg_type is None else (tuple(seg_type.shape), seg_type.dtype))
         ent = self.entries.get(key)
         if ent is None:
             if len(self.entries) > 4:
                 self.entries.clear()
-            ent = self.entries[key] = self._capture(imgs, tgts, bool_masked_pos, valid)
+            ent = self.entries[key] = self._capture(inputs)
         si, g, out = ent
-        si[0].copy_(imgs, non_blocking=True)
-        si[1].copy_(tgts, non_blocking=True)
-        si[2].copy_(bool_masked_pos, non_blocking=True)
-        si[3].copy_(valid, non_blocking=True)
+        for buf, t in zip(si, inputs):
+            buf.copy_(t, non_blocking=True)
         self.opt.graph_prepare()
         g.replay()
         return out
