@@ -207,8 +207,7 @@ def forward(model, imgs, tgts, mask_u8, valid, type_emb, merge_between_batch):
               "pk_dec_im2col_split3")
         _gemm(icol, wconv, kind=EPI_F32, bias=dp[0].bias, out=c1[b * Hh * Ww:(b + 1) * Hh * Ww])
         del icol
-    hp = torch.cat([dp[0].bias, dp[1].weight, dp[1].bias, dp[3].weight.reshape(-1), dp[3].bias,
-                    dp[3].bias.new_zeros(5)]).detach().float().contiguous()
+    hp = ops.pack_head_params(dp[0].bias, dp[1].weight, dp[1].bias, dp[3].weight, dp[3].bias)
     st = ops.loss_prep(tgts, mask_u8, valid, p)
     patch = torch.empty((B, N, p * p * 3), dtype=torch.float32, device=dev)
     numd = torch.zeros((B,), dtype=torch.float64, device=dev)

@@ -2,7 +2,7 @@
 
 Every parameter gradient of a training step is produced by exactly one backward stage (engine.py), so the stages
 write them straight into ONE zero-initialised fp32 slab laid out in the order backward produces them
-(decoder -> block 23 ... block 0 -> embedding).  What that buys:
+(decoder -> block 23 ... block 0 -> embedding), as the module's `grad_stages()` states it.  What that buys:
 
   * one memset per step instead of ~700 zero fills (stream-K weight-gradient GEMMs, LayerNorm / bias / rel-pos
     accumulators all need zero-initialised targets) - or none at all when `optim.FusedAdamW` clears each gradient as it
@@ -27,18 +27,7 @@ class GradArena:
     def __init__(self, model):
         dev = next(model.parameters()).device
         self.device = dev
-        groups = []   # production order
-        dec = [model.norm.weight, model.norm.bias, model.decoder_embed.weight, model.decoder_embed.bias]
-        dec += list(model.decoder_pred.parameters())
-        groups.append(("decoder", dec))
-        for i in reversed(range(len(model.blocks))):
-            groups.append((f"block{i}", list(model.blocks[i].parameters())))
-        emb = list(model.patch_embed.parameters()) + [model.mask_token, model.segment_token_x, model.segment_token_y]
-        for n in ("type_token_cls", "type_token_ins"):
-            if hasattr(model, n):
-                emb.append(getattr(model, n))
-        emb.append(model.pos_embed)
-        groups.append(("embed", emb))
+        groups = [(name, list(prm.values())) for name, prm in model.grad_stages().items()]   # production order
         self.offsets = {}
         self.group_ranges = []          # (name, start, end) in floats, production order
         off = 0

@@ -67,16 +67,11 @@ class Block(nn.Module):
         self.window_size = window_size
 
     def params(self):
+        """The block's parameters in BlockFn.ROLES order (BlockFn's parameter inputs)."""
         a, m = self.attn, self.mlp
         return (self.norm1.weight, self.norm1.bias, a.rel_pos_h, a.rel_pos_w, a.qkv.weight, a.qkv.bias,
                 a.proj.weight, a.proj.bias, self.norm2.weight, self.norm2.bias, m.fc1.weight, m.fc1.bias,
                 m.fc2.weight, m.fc2.bias)
-
-    ROLES = ("n1w", "n1b", "rel_h", "rel_w", "qkv_w", "qkv_b", "proj_w", "proj_b", "n2w", "n2b", "fc1_w", "fc1_b",
-             "fc2_w", "fc2_b")
-
-    def roles(self):
-        return dict(zip(self.ROLES, self.params()))
 
 
 class PatchEmbed(nn.Module):
@@ -243,6 +238,25 @@ class Painter(nn.Module):
         """Per-block view of the step's DropPath scales (tests replace this to replay the reference's CPU draws)."""
         return self._step_drops.get(i, (None, None))
 
+    def grad_stages(self):
+        """{stage: {role: parameter}} in backward production order (decoder, block N-1 ... block 0, embed), the roles
+        of each stage in the order of its Function's parameter inputs (engine.DecoderFn / BlockFn / EmbedFn.ROLES;
+        Painter has no type tokens "tc" / "ti").  The gradient arena lays its slab out in exactly this order, and
+        _run hands every stage its parameters from here."""
+        dp, pe = self.decoder_pred, self.patch_embed.proj
+        out = {"decoder": dict(zip(DecoderFn.ROLES, (self.norm.weight, self.norm.bias, self.decoder_embed.weight,
+                                                     self.decoder_embed.bias, dp[0].weight, dp[0].bias, dp[1].weight,
+                                                     dp[1].bias, dp[3].weight, dp[3].bias)))}
+        for i in reversed(range(len(self.blocks))):
+            out[f"block{i}"] = dict(zip(BlockFn.ROLES, self.blocks[i].params()))
+        emb = {"w": pe.weight, "b": pe.bias, "mt": self.mask_token, "sx": self.segment_token_x,
+               "sy": self.segment_token_y}
+        if self.seggpt:
+            emb.update(tc=self.type_token_cls, ti=self.type_token_ins)
+        emb["pe"] = self.pos_embed
+        out["embed"] = emb
+        return out
+
     def _type_inputs(self, B, seg_type, device):
         """(seg_type fp32 [B, 1] on the device, type_token_cls, type_token_ins) for SegGPT; Painter has no type tokens."""
         return None, None, None
@@ -280,24 +294,24 @@ class Painter(nn.Module):
             from . import accurate
             return accurate.forward(self, imgs.detach(), tgts.detach(), mask_u8, valid,
                                     self._type_emb(B, seg_type, dev), merge_between_batch)
-        pe = self.patch_embed.proj
-        # gradient arena + per-step token (engine.StageEnv): only when this forward can be followed by a backward that
-        # produces parameter gradients.  A fully frozen module (e.g. for prompt tuning) has none, and drops the arena
-        # of an earlier training phase.
+        # gradient arena + per-step token (engine.StageEnv): the arena only when this forward can be followed by a
+        # backward that produces parameter gradients.  A fully frozen module (e.g. for prompt tuning) has none, and
+        # drops the arena of an earlier training phase.
         trainable = any(q.requires_grad for q in self.parameters())
         if not trainable:
             self.__dict__.pop("_pk_arena", None)
         arena = get_arena(self) if torch.is_grad_enabled() and trainable else None
         link = engine.StepLink() if torch.is_grad_enabled() else None   # the block backwards' hand-off
         token = object()
-        emb_prm = {"w": pe.weight, "b": pe.bias, "mt": self.mask_token, "sx": self.segment_token_x,
-                   "sy": self.segment_token_y, "pe": self.pos_embed}
-        st, type_cls, type_ins = self._type_inputs(B, seg_type, dev)
-        if st is not None:
-            emb_prm.update(tc=type_cls, ti=type_ins)
-        z = EmbedFn.apply(imgs, tgts, mask_u8, st, pe.weight, pe.bias, self.mask_token, self.segment_token_x,
-                          self.segment_token_y, self.pos_embed, type_cls, type_ins, p, self.pretrain_use_cls_token,
-                          StageEnv(arena, token, "embed", emb_prm) if arena is not None else None)
+
+        def env(name, prm, below=None):
+            return StageEnv(arena, token, name, prm, below, link) if link is not None else None
+
+        stages = self.grad_stages()
+        emb = stages["embed"]
+        st, _, _ = self._type_inputs(B, seg_type, dev)
+        z = EmbedFn.apply(imgs, tgts, mask_u8, st, *(emb.get(r) for r in EmbedFn.ROLES), p,
+                          self.pretrain_use_cls_token, env("embed", emb))
         merge_idx = 2
         Bp = 2 * B
         taps = []
@@ -311,34 +325,25 @@ class Painter(nn.Module):
             if merge_between_batch >= 0 and i >= merge_between_batch:
                 ens_g, ens_p = (2, B) if merge_idx >= i else (1, B)
             da, dm = drops[i]
-            a = blk.attn
-            rel_h = engine.resize_rel_table(a.rel_pos_h, ws if ws > 0 else h)
-            rel_w = engine.resize_rel_table(a.rel_pos_w, ws if ws > 0 else w)
-            prm = blk.params()
-            env = None
-            if link is not None:
-                # hand-off: block i's dx is consumed only by block i-1's MLP branch (as bf16(DropPath scale * dx))
-                # unless block i-1's output also feeds the early merge or a decoder tap
-                below = None
-                if i > 0 and (i - 1) != merge_idx and (i - 1) not in (5, 11, 17, 23) and ens_g == 0:
-                    below = (self.blocks[i - 1].mlp.fc2.bias, drops[i - 1][1], N)
-                env = StageEnv(arena, token, f"block{i}", blk.roles(), below, link)
-            z = BlockFn.apply(z, da, dm, prm[0], prm[1], rel_h, rel_w, *prm[4:],
-                              (Bp, h, w, self.num_heads, blk.norm1.eps, ens_g, ens_p, ws), env)
+            prm = stages[f"block{i}"]
+            prm["rel_h"] = engine.resize_rel_table(prm["rel_h"], ws if ws > 0 else h)
+            prm["rel_w"] = engine.resize_rel_table(prm["rel_w"], ws if ws > 0 else w)
+            # hand-off: block i's dx is consumed only by block i-1's MLP branch (as bf16(DropPath scale * dx)) unless
+            # block i-1's output also feeds the early merge or a decoder tap
+            below = None
+            if i > 0 and (i - 1) != merge_idx and (i - 1) not in (5, 11, 17, 23) and ens_g == 0:
+                below = (self.blocks[i - 1].mlp.fc2.bias, drops[i - 1][1], N)
+            z = BlockFn.apply(z, da, dm, *prm.values(), (Bp, h, w, self.num_heads, blk.norm1.eps, ens_g, ens_p, ws),
+                              env(f"block{i}", prm, below))
             if i == merge_idx:
                 z = MergeFn.apply(z)
                 Bp = B
             if i in (5, 11, 17, 23):
                 taps.append(z)
-        dp = self.decoder_pred
-        dec_prm = {"norm_w": self.norm.weight, "norm_b": self.norm.bias, "dec_w": self.decoder_embed.weight,
-                   "dec_b": self.decoder_embed.bias, "c3_w": dp[0].weight, "c3_b": dp[0].bias, "ln_w": dp[1].weight,
-                   "ln_b": dp[1].bias, "c1_w": dp[3].weight, "c1_b": dp[3].bias}
-        loss, patch = DecoderFn.apply(taps[0], taps[1], taps[2], taps[3], self.norm.weight, self.norm.bias,
-                                      self.decoder_embed.weight, self.decoder_embed.bias, dp[0].weight, dp[0].bias,
-                                      dp[1].weight, dp[1].bias, dp[3].weight, dp[3].bias, tgts, mask_u8, valid,
+        dec = stages["decoder"]
+        loss, patch = DecoderFn.apply(*taps, tgts, *dec.values(), mask_u8, valid,
                                       (B, h, w, p, self.norm.eps, engine.LOSS_KINDS[self.loss_func], self.seggpt),
-                                      StageEnv(arena, token, "decoder", dec_prm) if arena is not None else None)
+                                      env("decoder", dec))
         return loss.reshape(()), patch
 
     def forward(self, imgs, tgts, bool_masked_pos=None, valid=None):

@@ -104,16 +104,18 @@ def relpos_table_bf16(table):
     return out
 
 
-def attn_fwd(qkv, th, tw, B, heads, h, w, need_lse=True, save_rel=False):
+def attn_fwd(qkv, th, tw, B, heads, h, w, save_rel=False):
     """Fused attention forward. qkv: bf16 [B*h*w, 3*heads*64]; th/tw: padded bf16 tables for an (h, w) grid.
-    Returns (out bf16 [B*h*w, heads*64], lse fp32 [B*heads, h*w] in the log2 domain); with save_rel=True (training) a
-    third value: the (relh, relw) bias-row buffers the forward keeps for `attn_bwd(..., rel=...)`."""
+    Returns (out bf16 [B*h*w, heads*64], lse fp32 [B*heads, h*w] in the log2 domain); with save_rel=True a third
+    value: the (relh, relw) bias-row buffers the forward keeps for `attn_bwd(..., rel=...)`.  The module does not use
+    that pair (72 MB of extra saved activations per block application at batch 8, to save one small kernel); the
+    tests compare the recomputing backward against it."""
     _req(qkv, torch.bfloat16, "qkv")
     N, C = h * w, heads * 64
     assert qkv.is_contiguous() and tuple(qkv.shape) == (B * N, 3 * C)
     assert th.shape[0] >= 2 * h - 1 and tw.shape[0] >= 2 * w - 1
     out = torch.empty((B * N, C), dtype=torch.bfloat16, device=qkv.device)
-    lse = torch.empty((B * heads, N), dtype=torch.float32, device=qkv.device) if (need_lse or save_rel) else None
+    lse = torch.empty((B * heads, N), dtype=torch.float32, device=qkv.device)
     if save_rel:
         Np = (N + 127) // 128 * 128     # whole 128-query tiles, query row innermost
         relh = torch.empty((B * heads * Np * h,), dtype=torch.float32, device=qkv.device)
@@ -142,8 +144,7 @@ def attn_fwd_split3(qkv, th, tw, B, heads, h, w):
     return out
 
 
-def attn_bwd(qkv, out, dout, lse, th, tw, B, heads, h, w, L_h=None, L_w=None, dT_out=None, rel=None,
-             table_grads=True):
+def attn_bwd(qkv, out, dout, lse, th, tw, B, heads, h, w, dT_out=None, rel=None, table_grads=True):
     """Fused attention backward.  Returns (dqkv bf16 [B*N, 3C], dTh fp32 [2h-1, 64], dTw fp32 [2w-1, 64]).
     rel: the (relh, relw) buffers of `attn_fwd(..., save_rel=True)` on the same operands (the dQ kernel then loads its
     bias rows instead of recomputing them).  table_grads=False (frozen tables): dTh = dTw = None, the table-gradient
@@ -379,6 +380,17 @@ def loss_prep(tgts, mask_u8, valid, p):
     check(lib().pk_loss_prep(_ptr(tgts), _ptr(mask_u8), mask_u8.shape[0], _ptr(valid), _ptr(stats), B, H, W, p,
                              _stream()), "pk_loss_prep")
     return stats
+
+
+# The decoder head's packed parameter vector (pk_decoder_head_fwd / pk_decoder_head_bwd / pk_head_f32), fp32 [392]:
+# conv3x3 bias [64] | LayerNorm2D weight [64] | bias [64] | conv1x1 weight [3*64] | conv1x1 bias [3] | 5 zeros.  The
+# head backward returns the gradients of the last four in the same slices (the conv3x3 bias gradient is a column sum
+# of dc1 instead).
+HEAD_SLICES = {"ln_w": slice(64, 128), "ln_b": slice(128, 192), "c1_w": slice(192, 384), "c1_b": slice(384, 387)}
+
+
+def pack_head_params(c3_b, ln_w, ln_b, c1_w, c1_b):
+    return torch.cat([c3_b, ln_w, ln_b, c1_w.reshape(-1), c1_b, c1_b.new_zeros(5)]).contiguous()
 
 
 def decoder_head_fwd(g_nhwc, wf, head_params, tgts, mask_u8, valid, p, loss_kind):

@@ -3,6 +3,7 @@ gradient averaging == DDP == mean of the per-rank gradients (computed with the t
 import os
 import socket
 
+import pytest
 import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
@@ -55,12 +56,13 @@ def test_gloo_world2_gradient_average_and_timing(tmp_path):
     assert len(set(r["seeds"])) == 2 and r["differ"]      # ranks really process different batches
 
 
-def _tiny_module():
+def _tiny_module(seggpt=False):
     from functools import partial
-    from painter_b200 import models_painter
+    from painter_b200 import models_painter, models_seggpt
     torch.manual_seed(0)
-    return models_painter.Painter(img_size=(64, 32), embed_dim=64, num_heads=1, decoder_embed_dim=64, use_rel_pos=True,
-                                  depth=24, norm_layer=partial(torch.nn.LayerNorm, eps=1e-6))
+    cls = models_seggpt.SegGPT if seggpt else models_painter.Painter
+    return cls(img_size=(64, 32), embed_dim=64, num_heads=1, decoder_embed_dim=64, use_rel_pos=True, depth=24,
+               norm_layer=partial(torch.nn.LayerNorm, eps=1e-6))
 
 
 def _sync_worker(rank, world, port, out):
@@ -134,3 +136,36 @@ def test_arena_layout_follows_backward_production_order():
     assert all(s1[1] <= s2[0] for s1, s2 in zip(spans, spans[1:]))          # no overlap
     b = GradSync.plan(a.group_ranges, 0.05)
     assert b[0][0] == 0 and b[-1][1] == a.total and all(x[1] == y[0] for x, y in zip(b, b[1:]))
+
+
+BLOCK_PARAMS = ("norm1.weight", "norm1.bias", "attn.rel_pos_h", "attn.rel_pos_w", "attn.qkv.weight", "attn.qkv.bias",
+                "attn.proj.weight", "attn.proj.bias", "norm2.weight", "norm2.bias", "mlp.fc1.weight", "mlp.fc1.bias",
+                "mlp.fc2.weight", "mlp.fc2.bias")
+
+
+@pytest.mark.parametrize("seggpt", [False, True])
+def test_arena_slab_layout_is_pinned(seggpt):
+    """Every parameter's offset and every group's range in the gradient slab, spelled out by parameter name: GradSync
+    buckets and FusedAdamW chunks are cut along them."""
+    from painter_b200.arena import GradArena
+    m = _tiny_module(seggpt)
+    groups = [("decoder", ["norm.weight", "norm.bias", "decoder_embed.weight", "decoder_embed.bias",
+                           "decoder_pred.0.weight", "decoder_pred.0.bias", "decoder_pred.1.weight",
+                           "decoder_pred.1.bias", "decoder_pred.3.weight", "decoder_pred.3.bias"])]
+    groups += [(f"block{i}", [f"blocks.{i}.{n}" for n in BLOCK_PARAMS]) for i in range(23, -1, -1)]
+    groups.append(("embed", ["patch_embed.proj.weight", "patch_embed.proj.bias", "mask_token", "segment_token_x",
+                             "segment_token_y"] + (["type_token_cls", "type_token_ins"] if seggpt else []) +
+                   ["pos_embed"]))
+    prm = dict(m.named_parameters())
+    assert sorted(prm) == sorted(n for _, names in groups for n in names)
+    want_offsets, want_ranges, off = {}, [], 0
+    for name, names in groups:
+        start = off
+        for n in names:
+            want_offsets[n] = off
+            off += -(-prm[n].numel() // 64) * 64
+        want_ranges.append((name, start, off))
+    a = GradArena(m)
+    assert a.group_ranges == want_ranges
+    assert {n: a.offsets[id(p)][0] for n, p in prm.items()} == want_offsets
+    assert a.total == off == (5525248 if seggpt else 5525120)
