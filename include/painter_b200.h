@@ -281,7 +281,21 @@ int pk_set_pdl(int on);
  *                       thread or when OH + OW <= 128), else its generic one
  *  pk_nearest_u8        dst uint8 [OH,OW,3] = uint8(int(nearest(src))) (painter_inference_pano_inst.py,
  *                       painter_inference_pose.py run_one_image); cl_form selects torch-CPU's channels-last source
- *                       index (it takes that kernel when OH + OW <= 128), else its generic one                      */
+ *                       index (it takes that kernel when OH + OW <= 128), else its generic one
+ * pk_stitch_normalize takes any number of members (launched in chunks of 16).
+ * Batched inference (many canvases per forward, painter_inference.run_batch, seggpt_engine.segment_batch):
+ *  pk_denorm_bottom_batched  out fp64 [B, h*p/2, w*p, 3]: pk_denorm_bottom of samples 0, src_stride, 2 src_stride, ..
+ *                       of patch; bin (nullable, finish 0 only) fp32 [B, h*p/2, w*p] as in pk_seg_postprocess
+ *  pk_finish_ragged     one launch finishing n images of different output sizes from src fp64 [*, SH, SW, 3] with the
+ *                       per-pixel code of the single-image kernel of `op` (PK_FIN_*).  items: int32 device table, one
+ *                       row of PK_RAG_FIELDS per image: [src sample, OH, OW, cl_form, offset lo, hi]; the image's
+ *                       output starts at dst + offset (elements of the op's output type: uint8, int32 for the depth,
+ *                       fp64 for the bicubic) and, for the blend, its source image uint8 [OH, OW, 3] at image + offset
+ *                       (image is null for every other op).  cl_form as in the single-image call (nearest_u8, depth).
+ *                       max_pix >= every OH * OW sizes the grid.                                                    */
+enum { PK_RAG_FIELDS = 6 };
+enum { PK_FIN_BILINEAR_U8 = 0, PK_FIN_NEAREST_U8 = 1, PK_FIN_DEPTH = 2, PK_FIN_BICUBIC_F64 = 3,
+       PK_FIN_NEAREST_BLEND = 4 };
 int pk_stitch_normalize(const void* const* top, const int* top_dtype, const void* const* bottom,
                         const int* bottom_dtype, float* out, int P, int S, void* stream);
 int pk_nhwc_to_nchw_f32(const void* in, int in_is_f64, float* out, int n, int H, int W, void* stream);
@@ -293,6 +307,10 @@ int pk_denorm_bottom(const float* patch, double* out, int h, int w, int p, int f
 int pk_bicubic_f64(const double* src, int SH, int SW, double* dst, int OH, int OW, void* stream);
 int pk_depth_finish(const double* src, int SH, int SW, int32_t* dst, int OH, int OW, int cl_form, void* stream);
 int pk_nearest_u8(const double* src, int SH, int SW, uint8_t* dst, int OH, int OW, int cl_form, void* stream);
+int pk_denorm_bottom_batched(const float* patch, double* out, float* bin_or_null, int B, int src_stride, int h, int w,
+                             int p, int finish, void* stream);
+int pk_finish_ragged(int op, const double* src, int SH, int SW, const int* items, int n, int max_pix,
+                     const uint8_t* image, void* dst, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * fp32-accurate forward mode (north star: within 1e-5 of the reference's fp32 forward, the way

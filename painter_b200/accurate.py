@@ -28,6 +28,34 @@ def _pad64(n):
     return (n + 63) // 64 * 64
 
 
+def selected(model):
+    """Whether a forward of `model` called now runs this path (model.precision, see the module docstring)."""
+    prec = model.precision
+    return prec == "fp32" or (prec == "auto" and not torch.is_autocast_enabled("cuda") and
+                              not torch.is_grad_enabled())
+
+
+def workspace_bytes(model, B, H, W):
+    """Device memory a forward of B canvases [3, H, W] in this mode allocates at its peak, from the shapes: the global
+    blocks before the early merge (2B token grids) hold the per-(sample, head) score matrix and split operands of
+    `attention`, the rel-pos projections, the block's fp32 activations and the split qkv operand; the decoder (one
+    image's im2col at a time) needs less for the stock geometry but is counted in case it does not.  Includes the
+    weights' split copies when they are not cached yet."""
+    p, C, heads = model.patch_size, model.embed_dim, model.num_heads
+    h, w = H // p, W // p
+    N, Bp = h * w, 2 * B
+    Np = _pad64(N)
+    attn = Bp * heads * (N * 384 * 2 + Np * 384 * 2 + 6 * Np * 64 * 2 + N * Np * 4 + N * 6 * Np * 2 +
+                         N * (_pad64(2 * h - 1) + _pad64(2 * w - 1)) * 4)
+    blocks = attn + Bp * N * C * (4 + 4 + 12 + 12 + 4)          # z, u, split3(u), qkv, attention output
+    dd = model.decoder_embed_dim
+    dec = B * N * C * 4 * 8 + B * N * p * p * dd * 4 + B * H * W * 64 * 4 + H * W * 6 * 9 * dd * 2
+    need = max(blocks, dec)
+    if getattr(model.blocks[0].attn.qkv.weight, "_pk_split3", None) is None:
+        need += 12 * sum(q.numel() for q in model.parameters() if q.dim() >= 2)
+    return need
+
+
 def split3(x, side_b=False, gelu=False):
     """fp32 [M, K] (row stride free) -> bf16 [M, 6K] split operand (A-side or B-side term order)."""
     assert x.dtype == torch.float32 and x.dim() == 2 and x.stride(1) == 1
@@ -145,7 +173,7 @@ def block(z, blk, Bp, h, w, heads, eps, ens, ws_cache, rel_h, rel_w):
 
 
 @torch.no_grad()
-def forward(model, imgs, tgts, mask_u8, valid, type_emb, merge_between_batch):
+def forward(model, imgs, tgts, mask_u8, valid, type_emb, merge_between_batch, prompts_per_query=None):
     """(loss [()], patchify(pred) [B, N, p*p*3]) - Painter._run in fp32-accurate arithmetic."""
     from . import engine
     p = model.patch_size
@@ -172,9 +200,7 @@ def forward(model, imgs, tgts, mask_u8, valid, type_emb, merge_between_batch):
     ws_cache = {}
     Bp, merge_idx, taps = 2 * B, 2, []
     for i, blk in enumerate(model.blocks):
-        ens = (0, 0)
-        if merge_between_batch >= 0 and i >= merge_between_batch:
-            ens = (2, B) if merge_idx >= i else (1, B)
+        ens = model._ensemble(i, B, merge_between_batch, prompts_per_query, merge_idx)
         ws = blk.window_size
         rel_h = engine.resize_rel_table(blk.attn.rel_pos_h, ws if ws > 0 else h)
         rel_w = engine.resize_rel_table(blk.attn.rel_pos_w, ws if ws > 0 else w)

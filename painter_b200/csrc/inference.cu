@@ -29,11 +29,12 @@ __device__ __forceinline__ double load_unit(const void* src, int dtype, size_t i
 // canvas[p, c, y, x] (fp32 NCHW, [P, 3, 2S, S]) = ((y < S ? top[p] : bottom[p])[y % S, x, c] - mean[c]) / std[c]
 // top / bottom: per-member pointers to HWC images [S, S, 3] in [0,1] (or uint8); seggpt_engine.py:75-91 (stitch,
 // normalise), :29-34 (nhwc -> nchw, .float()).
+constexpr int kCanvasMembers = 16;
 struct CanvasSrc {
-  const void* top[16];
-  const void* bottom[16];
-  int top_dtype[16];
-  int bottom_dtype[16];
+  const void* top[kCanvasMembers];
+  const void* bottom[kCanvasMembers];
+  int top_dtype[kCanvasMembers];
+  int bottom_dtype[kCanvasMembers];
 };
 __global__ void __launch_bounds__(256)
 stitch_normalize_kernel(const CanvasSrc src, float* __restrict__ out, int P, int S) {
@@ -76,21 +77,25 @@ nhwc_to_nchw_f32_kernel(const void* __restrict__ in, int in_is_f64, float* __res
 //   kPlain     x                          sidd / lol / derain (no clip)
 enum DenormFinish { kClip255 = 0, kClip10000 = 1, kPlain = 2 };
 
-// out[y, x, c] (fp64 [H/2, W, 3]) = finish(pred_pixel(sample 0, y + H/2, x, c) * std[c] + mean[c])
-// patch: patchified prediction [B, h*w, p*p*3] fp32 (inner order (pr, pc, c), models_painter.py:355-368);
+// out[b, y, x, c] (fp64 [B, H/2, W, 3]) = finish(pred_pixel(sample b * src_stride, y + H/2, x, c) * std[c] + mean[c])
+// patch: patchified prediction [*, h*w, p*p*3] fp32 (inner order (pr, pc, c), models_painter.py:355-368);
 // = unpatchify -> 'nchw->nhwc' -> bottom half -> de-normalise (seggpt_engine.py:48-52).  Optionally (kClip255 only)
-// also writes bin[y, x] = (mean_c(out) > 128) (the video path's next-frame target, seggpt_engine.py:164-169).
+// also writes bin[b, y, x] = (mean_c(out) > 128) (the video path's next-frame target, seggpt_engine.py:164-169).
+// The single-image entry points run it with B = 1; every sample's pixels get the same arithmetic.
 template <int kFinish>
 __global__ void __launch_bounds__(256)
-seg_postprocess_kernel(const float* __restrict__ patch, double* __restrict__ out, float* __restrict__ bin, int h,
-                       int w, int p) {
+seg_postprocess_kernel(const float* __restrict__ patch, double* __restrict__ out, float* __restrict__ bin, int B,
+                       int src_stride, int h, int w, int p) {
   const int H = h * p, W = w * p, Hh = H / 2;
-  const size_t total = static_cast<size_t>(Hh) * W;
+  const size_t per = static_cast<size_t>(Hh) * W;
+  const size_t total = per * B;
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int x = static_cast<int>(i % W), y = static_cast<int>(i / W) + Hh;
+    const size_t b = i / per, j = i % per;
+    const int x = static_cast<int>(j % W), y = static_cast<int>(j / W) + Hh;
     const int ti = y / p, tj = x / p, pr = y % p, pc = x % p;
-    const float* src = patch + (static_cast<size_t>(ti) * w + tj) * (p * p * 3) + (pr * p + pc) * 3;
+    const float* src = patch + b * src_stride * (static_cast<size_t>(h) * w * p * p * 3) +
+                       (static_cast<size_t>(ti) * w + tj) * (p * p * 3) + (pr * p + pc) * 3;
     double s = 0.0;
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
@@ -119,21 +124,27 @@ __device__ __forceinline__ int nearest_idx(int dst, int in_size, int out_size) {
   return s < in_size - 1 ? s : in_size - 1;
 }
 // dst[y, x, c] (uint8 [OH, OW, 3]) = uint8(image[y, x, c] * (0.6 * nearest(seg)[y, x, c] / 255 + 0.4))
-// (seggpt_engine.py:97-102: F.interpolate(mode='nearest') to the original size, alpha blend, astype(uint8))
+// (seggpt_engine.py:97-102: F.interpolate(mode='nearest') to the original size, alpha blend, astype(uint8)).
+// The *_at functions compute output element i of one image; the single-image kernel and the ragged kernel
+// (ragged_finish_kernel) both call them, so a batched result is the single-image result.
+__device__ __forceinline__ void nearest_blend_at(const double* __restrict__ seg, int SH, int SW,
+                                                 const uint8_t* __restrict__ image, uint8_t* __restrict__ dst, int OH,
+                                                 int OW, size_t i) {
+  const int c = static_cast<int>(i % 3);
+  const size_t r = i / 3;
+  const int x = static_cast<int>(r % OW), y = static_cast<int>(r / OW);
+  const int sy = nearest_idx(y, SH, OH), sx = nearest_idx(x, SW, OW);
+  const double o = seg[(static_cast<size_t>(sy) * SW + sx) * 3 + c];
+  const double v = __dmul_rn(static_cast<double>(image[i]), __dadd_rn(__dmul_rn(0.6, o) / 255.0, 0.4));
+  dst[i] = static_cast<uint8_t>(v);   // numpy astype(uint8): truncation (values are within [0, 255])
+}
 __global__ void __launch_bounds__(256)
 nearest_blend_kernel(const double* __restrict__ seg, int SH, int SW, const uint8_t* __restrict__ image,
                      uint8_t* __restrict__ dst, int OH, int OW) {
   const size_t total = static_cast<size_t>(OH) * OW * 3;
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int c = static_cast<int>(i % 3);
-    const size_t r = i / 3;
-    const int x = static_cast<int>(r % OW), y = static_cast<int>(r / OW);
-    const int sy = nearest_idx(y, SH, OH), sx = nearest_idx(x, SW, OW);
-    const double o = seg[(static_cast<size_t>(sy) * SW + sx) * 3 + c];
-    const double v = __dmul_rn(static_cast<double>(image[i]), __dadd_rn(__dmul_rn(0.6, o) / 255.0, 0.4));
-    dst[i] = static_cast<uint8_t>(v);   // numpy astype(uint8): truncation (values are within [0, 255])
-  }
+       i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    nearest_blend_at(seg, SH, SW, image, dst, OH, OW, i);
 }
 
 // One axis of ATen's linear interpolation (align_corners=False, scale = in / out from the sizes):
@@ -164,21 +175,24 @@ __device__ __forceinline__ LinearTap linear_tap(int dst, int in_size, int out_si
 
 // dst[y, x, c] (uint8 [OH, OW, 3]) = uint8(int(bilinear(seg)[y, x, c]))   (painter_inference_segm.py:89-92:
 // F.interpolate(mode='bilinear', align_corners=False) on the float64 tensor, .int(), astype(uint8))
+__device__ __forceinline__ void bilinear_u8_at(const double* __restrict__ seg, int SH, int SW,
+                                               uint8_t* __restrict__ dst, int OH, int OW, size_t i) {
+  const double sch = static_cast<double>(SH) / OH, scw = static_cast<double>(SW) / OW;
+  const int c = static_cast<int>(i % 3);
+  const size_t r = i / 3;
+  const int x = static_cast<int>(r % OW), y = static_cast<int>(r / OW);
+  const LinearTap ty = linear_tap(y, SH, OH, sch), tx = linear_tap(x, SW, OW, scw);
+  auto at = [&](int yy, int xx) { return seg[(static_cast<size_t>(yy) * SW + xx) * 3 + c]; };
+  const double v = ty.l0 * (tx.l0 * at(ty.i0, tx.i0) + tx.l1 * at(ty.i0, tx.i1)) +
+                   ty.l1 * (tx.l0 * at(ty.i1, tx.i0) + tx.l1 * at(ty.i1, tx.i1));
+  dst[i] = static_cast<uint8_t>(static_cast<int>(v));
+}
 __global__ void __launch_bounds__(256)
 bilinear_u8_kernel(const double* __restrict__ seg, int SH, int SW, uint8_t* __restrict__ dst, int OH, int OW) {
   const size_t total = static_cast<size_t>(OH) * OW * 3;
-  const double sch = static_cast<double>(SH) / OH, scw = static_cast<double>(SW) / OW;
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int c = static_cast<int>(i % 3);
-    const size_t r = i / 3;
-    const int x = static_cast<int>(r % OW), y = static_cast<int>(r / OW);
-    const LinearTap ty = linear_tap(y, SH, OH, sch), tx = linear_tap(x, SW, OW, scw);
-    auto at = [&](int yy, int xx) { return seg[(static_cast<size_t>(yy) * SW + xx) * 3 + c]; };
-    const double v = ty.l0 * (tx.l0 * at(ty.i0, tx.i0) + tx.l1 * at(ty.i0, tx.i1)) +
-                     ty.l1 * (tx.l0 * at(ty.i1, tx.i0) + tx.l1 * at(ty.i1, tx.i1));
-    dst[i] = static_cast<uint8_t>(static_cast<int>(v));
-  }
+       i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    bilinear_u8_at(seg, SH, SW, dst, OH, OW, i);
 }
 
 // dst[y, x] (int32 [OH, OW]) = int(mean_c(bilinear(src)[y, x, c]))   (nyuv2_depth/painter_inference_depth.py:
@@ -187,36 +201,39 @@ bilinear_u8_kernel(const double* __restrict__ seg, int SH, int SW, uint8_t* __re
 //   cl_form = 0 (its generic kernel)        (v00 l0x + v01 l1x) l0y + (v10 l0x + v11 l1x) l1y
 //   cl_form = 1 (its channels-last kernel)  v00 (l0y l0x) + v01 (l0y l1x) + v10 (l1y l0x) + v11 (l1y l1x), left to right
 // The mean is torch's sum over the 3 channels in order, then / 3.
+__device__ __forceinline__ void depth_finish_at(const double* __restrict__ src, int SH, int SW,
+                                                int32_t* __restrict__ dst, int OH, int OW, int cl_form, size_t i) {
+  const double sch = static_cast<double>(SH) / OH, scw = static_cast<double>(SW) / OW;
+  const int x = static_cast<int>(i % OW), y = static_cast<int>(i / OW);
+  const LinearTap ty = linear_tap(y, SH, OH, sch), tx = linear_tap(x, SW, OW, scw);
+  const double* r0 = src + static_cast<size_t>(ty.i0) * SW * 3;
+  const double* r1 = src + static_cast<size_t>(ty.i1) * SW * 3;
+  const double w00 = __dmul_rn(ty.l0, tx.l0), w01 = __dmul_rn(ty.l0, tx.l1);
+  const double w10 = __dmul_rn(ty.l1, tx.l0), w11 = __dmul_rn(ty.l1, tx.l1);
+  double s = 0.0;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const double v00 = r0[tx.i0 * 3 + c], v01 = r0[tx.i1 * 3 + c];
+    const double v10 = r1[tx.i0 * 3 + c], v11 = r1[tx.i1 * 3 + c];
+    double v;
+    if (cl_form) {
+      v = __fma_rn(v11, w11, __fma_rn(v10, w10, __fma_rn(v00, w00, __dmul_rn(v01, w01))));
+    } else {
+      const double t0 = __fma_rn(v00, tx.l0, __dmul_rn(v01, tx.l1));
+      const double t1 = __fma_rn(v10, tx.l0, __dmul_rn(v11, tx.l1));
+      v = __fma_rn(t0, ty.l0, __dmul_rn(t1, ty.l1));
+    }
+    s = c == 0 ? v : __dadd_rn(s, v);
+  }
+  dst[i] = static_cast<int32_t>(__ddiv_rn(s, 3.0));   // .int(): truncation (values are within [0, 10000])
+}
 __global__ void __launch_bounds__(256)
 depth_finish_kernel(const double* __restrict__ src, int SH, int SW, int32_t* __restrict__ dst, int OH, int OW,
                     int cl_form) {
   const size_t total = static_cast<size_t>(OH) * OW;
-  const double sch = static_cast<double>(SH) / OH, scw = static_cast<double>(SW) / OW;
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int x = static_cast<int>(i % OW), y = static_cast<int>(i / OW);
-    const LinearTap ty = linear_tap(y, SH, OH, sch), tx = linear_tap(x, SW, OW, scw);
-    const double* r0 = src + static_cast<size_t>(ty.i0) * SW * 3;
-    const double* r1 = src + static_cast<size_t>(ty.i1) * SW * 3;
-    const double w00 = __dmul_rn(ty.l0, tx.l0), w01 = __dmul_rn(ty.l0, tx.l1);
-    const double w10 = __dmul_rn(ty.l1, tx.l0), w11 = __dmul_rn(ty.l1, tx.l1);
-    double s = 0.0;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      const double v00 = r0[tx.i0 * 3 + c], v01 = r0[tx.i1 * 3 + c];
-      const double v10 = r1[tx.i0 * 3 + c], v11 = r1[tx.i1 * 3 + c];
-      double v;
-      if (cl_form) {
-        v = __fma_rn(v11, w11, __fma_rn(v10, w10, __fma_rn(v00, w00, __dmul_rn(v01, w01))));
-      } else {
-        const double t0 = __fma_rn(v00, tx.l0, __dmul_rn(v01, tx.l1));
-        const double t1 = __fma_rn(v10, tx.l0, __dmul_rn(v11, tx.l1));
-        v = __fma_rn(t0, ty.l0, __dmul_rn(t1, ty.l1));
-      }
-      s = c == 0 ? v : __dadd_rn(s, v);
-    }
-    dst[i] = static_cast<int32_t>(__ddiv_rn(s, 3.0));   // .int(): truncation (values are within [0, 10000])
-  }
+       i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    depth_finish_at(src, SH, SW, dst, OH, OW, cl_form, i);
 }
 
 // ATen's nearest source index in its generic kernel (HelperInterpNearest): scale = double(in) / out, then
@@ -230,20 +247,23 @@ __device__ __forceinline__ int nearest_idx_generic(int dst, int in_size, double 
 // mmpose_custom/painter_inference_pose.py: F.interpolate(mode='nearest') on the float64 tensor, .int(), astype(uint8)).
 // cl_form = 1: torch-CPU's channels-last kernel (which it takes for 3 channels when OH + OW <= 128), else its generic
 // kernel; the two compute the source index differently.
+__device__ __forceinline__ void nearest_u8_at(const double* __restrict__ src, int SH, int SW,
+                                              uint8_t* __restrict__ dst, int OH, int OW, int cl_form, size_t i) {
+  const double sch = static_cast<double>(SH) / OH, scw = static_cast<double>(SW) / OW;
+  const int c = static_cast<int>(i % 3);
+  const size_t r = i / 3;
+  const int x = static_cast<int>(r % OW), y = static_cast<int>(r / OW);
+  const int sy = cl_form ? nearest_idx(y, SH, OH) : nearest_idx_generic(y, SH, sch);
+  const int sx = cl_form ? nearest_idx(x, SW, OW) : nearest_idx_generic(x, SW, scw);
+  dst[i] = static_cast<uint8_t>(static_cast<int>(src[(static_cast<size_t>(sy) * SW + sx) * 3 + c]));
+}
 __global__ void __launch_bounds__(256)
 nearest_u8_kernel(const double* __restrict__ src, int SH, int SW, uint8_t* __restrict__ dst, int OH, int OW,
                   int cl_form) {
   const size_t total = static_cast<size_t>(OH) * OW * 3;
-  const double sch = static_cast<double>(SH) / OH, scw = static_cast<double>(SW) / OW;
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int c = static_cast<int>(i % 3);
-    const size_t r = i / 3;
-    const int x = static_cast<int>(r % OW), y = static_cast<int>(r / OW);
-    const int sy = cl_form ? nearest_idx(y, SH, OH) : nearest_idx_generic(y, SH, sch);
-    const int sx = cl_form ? nearest_idx(x, SW, OW) : nearest_idx_generic(x, SW, scw);
-    dst[i] = static_cast<uint8_t>(static_cast<int>(src[(static_cast<size_t>(sy) * SW + sx) * 3 + c]));
-  }
+       i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    nearest_u8_at(src, SH, SW, dst, OH, OW, cl_form, i);
 }
 
 // ATen's cubic convolution weights (get_cubic_upsample_coefficients, A = -0.75) of the 4 taps around a source
@@ -292,26 +312,58 @@ __device__ __forceinline__ double cubic_sum(const double v[4], const double w[4]
 // dst[y, x, c] (fp64 [OH, OW, 3]) = bicubic(src)[y, x, c]   (sidd / lol / derain painter_inference_*.py:
 // F.interpolate(mode='bicubic', align_corners=False) on the float64 tensor, no clipping).  As in ATen, each of the 4
 // source rows is first summed along x, then the 4 row sums along y.
+__device__ __forceinline__ void bicubic_f64_at(const double* __restrict__ src, int SH, int SW,
+                                               double* __restrict__ dst, int OH, int OW, size_t i) {
+  const double sch = static_cast<double>(SH) / OH, scw = static_cast<double>(SW) / OW;
+  const int c = static_cast<int>(i % 3);
+  const size_t r = i / 3;
+  const int x = static_cast<int>(r % OW), y = static_cast<int>(r / OW);
+  const CubicTaps ky = cubic_taps(y, SH, sch), kx = cubic_taps(x, SW, scw);
+  double rows[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const double* row = src + static_cast<size_t>(ky.idx[j]) * SW * 3 + c;
+    double v[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) v[k] = row[kx.idx[k] * 3];
+    rows[j] = cubic_sum(v, kx.w);
+  }
+  dst[i] = cubic_sum(rows, ky.w);
+}
 __global__ void __launch_bounds__(256)
 bicubic_f64_kernel(const double* __restrict__ src, int SH, int SW, double* __restrict__ dst, int OH, int OW) {
   const size_t total = static_cast<size_t>(OH) * OW * 3;
-  const double sch = static_cast<double>(SH) / OH, scw = static_cast<double>(SW) / OW;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    bicubic_f64_at(src, SH, SW, dst, OH, OW, i);
+}
+
+// Ragged finish of a batch: one CTA row (blockIdx.y) per descriptor row [src sample, OH, OW, cl_form, offset lo, hi]
+// (PK_RAG_FIELDS), grid-stride over that image's output elements.  src sample s is src + s * SH * SW * 3; the image's
+// output starts at dst + offset (elements of the output type), and for the blend the source image at image + offset.
+template <int kOp>
+__global__ void __launch_bounds__(256)
+ragged_finish_kernel(const double* __restrict__ src, int SH, int SW, const int* __restrict__ items,
+                     const uint8_t* __restrict__ image, void* __restrict__ dst) {
+  const int* it = items + static_cast<size_t>(blockIdx.y) * PK_RAG_FIELDS;
+  const int OH = it[1], OW = it[2], cl_form = it[3];
+  const size_t off = static_cast<size_t>(static_cast<uint32_t>(it[4])) |
+                     (static_cast<size_t>(static_cast<uint32_t>(it[5])) << 32);
+  const double* s = src + static_cast<size_t>(it[0]) * SH * SW * 3;
+  const size_t total = static_cast<size_t>(OH) * OW * (kOp == PK_FIN_DEPTH ? 1 : 3);
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int c = static_cast<int>(i % 3);
-    const size_t r = i / 3;
-    const int x = static_cast<int>(r % OW), y = static_cast<int>(r / OW);
-    const CubicTaps ky = cubic_taps(y, SH, sch), kx = cubic_taps(x, SW, scw);
-    double rows[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const double* row = src + static_cast<size_t>(ky.idx[j]) * SW * 3 + c;
-      double v[4];
-#pragma unroll
-      for (int k = 0; k < 4; ++k) v[k] = row[kx.idx[k] * 3];
-      rows[j] = cubic_sum(v, kx.w);
+    if constexpr (kOp == PK_FIN_BILINEAR_U8) {
+      bilinear_u8_at(s, SH, SW, static_cast<uint8_t*>(dst) + off, OH, OW, i);
+    } else if constexpr (kOp == PK_FIN_NEAREST_U8) {
+      nearest_u8_at(s, SH, SW, static_cast<uint8_t*>(dst) + off, OH, OW, cl_form, i);
+    } else if constexpr (kOp == PK_FIN_DEPTH) {
+      depth_finish_at(s, SH, SW, static_cast<int32_t*>(dst) + off, OH, OW, cl_form, i);
+    } else if constexpr (kOp == PK_FIN_BICUBIC_F64) {
+      bicubic_f64_at(s, SH, SW, static_cast<double*>(dst) + off, OH, OW, i);
+    } else {
+      nearest_blend_at(s, SH, SW, image + off, static_cast<uint8_t*>(dst) + off, OH, OW, i);
     }
-    dst[i] = cubic_sum(rows, ky.w);
   }
 }
 
@@ -321,26 +373,45 @@ static inline int stream_grid(size_t total) {
   return static_cast<int>(g < 1 ? 1 : (g > cap ? cap : g));
 }
 
+static int denorm_launch(const float* patch, double* out, float* bin, int B, int src_stride, int h, int w, int p,
+                         int finish, void* stream, const char* name) {
+  const size_t total = static_cast<size_t>(B) * h * p / 2 * w * p;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (finish == kClip255)
+    seg_postprocess_kernel<kClip255><<<stream_grid(total), 256, 0, st>>>(patch, out, bin, B, src_stride, h, w, p);
+  else if (finish == kClip10000)
+    seg_postprocess_kernel<kClip10000><<<stream_grid(total), 256, 0, st>>>(patch, out, bin, B, src_stride, h, w, p);
+  else
+    seg_postprocess_kernel<kPlain><<<stream_grid(total), 256, 0, st>>>(patch, out, bin, B, src_stride, h, w, p);
+  PK_LAUNCH_CHECK(name);
+  return 0;
+}
+
 }  // namespace pk
 
 using namespace pk;
 
 extern "C" int pk_stitch_normalize(const void* const* top, const int* top_dtype, const void* const* bottom,
                                    const int* bottom_dtype, float* out, int P, int S, void* stream) {
-  PK_CHECK(top && bottom && top_dtype && bottom_dtype && out && P >= 1 && P <= 16 && S > 0,
-           "pk_stitch_normalize: bad arguments (1 <= P <= 16)");
-  CanvasSrc src;
-  for (int p = 0; p < P; ++p) {
+  PK_CHECK(top && bottom && top_dtype && bottom_dtype && out && P >= 1 && S > 0, "pk_stitch_normalize: bad arguments");
+  for (int p = 0; p < P; ++p)
     PK_CHECK(top[p] && bottom[p] && top_dtype[p] >= 0 && top_dtype[p] <= 2 && bottom_dtype[p] >= 0 &&
                  bottom_dtype[p] <= 2, "pk_stitch_normalize: bad member %d", p);
-    src.top[p] = top[p];
-    src.bottom[p] = bottom[p];
-    src.top_dtype[p] = top_dtype[p];
-    src.bottom_dtype[p] = bottom_dtype[p];
+  // the member pointers travel as a kernel parameter of kCanvasMembers entries: one launch per chunk of members
+  const size_t per = static_cast<size_t>(3) * 2 * S * S;
+  for (int p0 = 0; p0 < P; p0 += kCanvasMembers) {
+    const int n = P - p0 < kCanvasMembers ? P - p0 : kCanvasMembers;
+    CanvasSrc src;
+    for (int p = 0; p < n; ++p) {
+      src.top[p] = top[p0 + p];
+      src.bottom[p] = bottom[p0 + p];
+      src.top_dtype[p] = top_dtype[p0 + p];
+      src.bottom_dtype[p] = bottom_dtype[p0 + p];
+    }
+    stitch_normalize_kernel<<<stream_grid(n * per), 256, 0, static_cast<cudaStream_t>(stream)>>>(src, out + p0 * per, n,
+                                                                                                  S);
+    PK_LAUNCH_CHECK("pk_stitch_normalize");
   }
-  const size_t total = static_cast<size_t>(P) * 3 * 2 * S * S;
-  stitch_normalize_kernel<<<stream_grid(total), 256, 0, static_cast<cudaStream_t>(stream)>>>(src, out, P, S);
-  PK_LAUNCH_CHECK("pk_stitch_normalize");
   return 0;
 }
 
@@ -358,7 +429,7 @@ extern "C" int pk_seg_postprocess(const float* patch, double* out, float* bin_or
   PK_CHECK(patch && out && h > 0 && w > 0 && p > 0 && h % 2 == 0, "pk_seg_postprocess: bad arguments");
   const size_t total = static_cast<size_t>(h) * p / 2 * w * p;
   seg_postprocess_kernel<kClip255><<<stream_grid(total), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      patch, out, bin_or_null, h, w, p);
+      patch, out, bin_or_null, 1, 1, h, w, p);
   PK_LAUNCH_CHECK("pk_seg_postprocess");
   return 0;
 }
@@ -366,16 +437,15 @@ extern "C" int pk_seg_postprocess(const float* patch, double* out, float* bin_or
 extern "C" int pk_denorm_bottom(const float* patch, double* out, int h, int w, int p, int finish, void* stream) {
   PK_CHECK(patch && out && h > 0 && w > 0 && p > 0 && h % 2 == 0 && finish >= kClip255 && finish <= kPlain,
            "pk_denorm_bottom: bad arguments");
-  const size_t total = static_cast<size_t>(h) * p / 2 * w * p;
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (finish == kClip255)
-    seg_postprocess_kernel<kClip255><<<stream_grid(total), 256, 0, st>>>(patch, out, nullptr, h, w, p);
-  else if (finish == kClip10000)
-    seg_postprocess_kernel<kClip10000><<<stream_grid(total), 256, 0, st>>>(patch, out, nullptr, h, w, p);
-  else
-    seg_postprocess_kernel<kPlain><<<stream_grid(total), 256, 0, st>>>(patch, out, nullptr, h, w, p);
-  PK_LAUNCH_CHECK("pk_denorm_bottom");
-  return 0;
+  return denorm_launch(patch, out, nullptr, 1, 1, h, w, p, finish, stream, "pk_denorm_bottom");
+}
+
+extern "C" int pk_denorm_bottom_batched(const float* patch, double* out, float* bin_or_null, int B, int src_stride,
+                                        int h, int w, int p, int finish, void* stream) {
+  PK_CHECK(patch && out && B >= 1 && src_stride >= 1 && h > 0 && w > 0 && p > 0 && h % 2 == 0 && finish >= kClip255 &&
+               finish <= kPlain, "pk_denorm_bottom_batched: bad arguments");
+  PK_CHECK(!bin_or_null || finish == kClip255, "pk_denorm_bottom_batched: the binarised mask needs finish 0 (x 255)");
+  return denorm_launch(patch, out, bin_or_null, B, src_stride, h, w, p, finish, stream, "pk_denorm_bottom_batched");
 }
 
 extern "C" int pk_nearest_blend(const double* seg, int SH, int SW, const uint8_t* image, uint8_t* dst, int OH, int OW,
@@ -418,5 +488,39 @@ extern "C" int pk_nearest_u8(const double* src, int SH, int SW, uint8_t* dst, in
   nearest_u8_kernel<<<stream_grid(static_cast<size_t>(OH) * OW * 3), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       src, SH, SW, dst, OH, OW, cl_form != 0);
   PK_LAUNCH_CHECK("pk_nearest_u8");
+  return 0;
+}
+
+extern "C" int pk_finish_ragged(int op, const double* src, int SH, int SW, const int* items, int n, int max_pix,
+                                const uint8_t* image, void* dst, void* stream) {
+  PK_CHECK(src && items && dst && SH > 0 && SW > 0 && n >= 1 && n <= 65535 && max_pix > 0,
+           "pk_finish_ragged: bad arguments (1 <= n <= 65535 images, max_pix > 0)");
+  PK_CHECK(op >= PK_FIN_BILINEAR_U8 && op <= PK_FIN_NEAREST_BLEND, "pk_finish_ragged: unknown op %d", op);
+  PK_CHECK((op == PK_FIN_NEAREST_BLEND) == (image != nullptr),
+           "pk_finish_ragged: the source images are given for the blend (op %d) and only for it", PK_FIN_NEAREST_BLEND);
+  // max_pix only sizes the grid (every loop is grid-stride): CTAs per image cover the largest image's elements
+  const size_t per = static_cast<size_t>(max_pix) * (op == PK_FIN_DEPTH ? 1 : 3);
+  const size_t cap = static_cast<size_t>(sm_count()) * 16;
+  size_t gx = (per + 255) / 256, gcap = (cap + n - 1) / n;
+  gx = gx < gcap ? gx : gcap;
+  const dim3 grid(static_cast<unsigned>(gx < 1 ? 1 : gx), static_cast<unsigned>(n));
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  switch (op) {
+    case PK_FIN_BILINEAR_U8:
+      ragged_finish_kernel<PK_FIN_BILINEAR_U8><<<grid, 256, 0, st>>>(src, SH, SW, items, image, dst);
+      break;
+    case PK_FIN_NEAREST_U8:
+      ragged_finish_kernel<PK_FIN_NEAREST_U8><<<grid, 256, 0, st>>>(src, SH, SW, items, image, dst);
+      break;
+    case PK_FIN_DEPTH:
+      ragged_finish_kernel<PK_FIN_DEPTH><<<grid, 256, 0, st>>>(src, SH, SW, items, image, dst);
+      break;
+    case PK_FIN_BICUBIC_F64:
+      ragged_finish_kernel<PK_FIN_BICUBIC_F64><<<grid, 256, 0, st>>>(src, SH, SW, items, image, dst);
+      break;
+    default:
+      ragged_finish_kernel<PK_FIN_NEAREST_BLEND><<<grid, 256, 0, st>>>(src, SH, SW, items, image, dst);
+  }
+  PK_LAUNCH_CHECK("pk_finish_ragged");
   return 0;
 }

@@ -265,7 +265,20 @@ class Painter(nn.Module):
         st, cls, ins = self._type_inputs(B, seg_type, device)
         return None if st is None else engine.type_embedding(st, cls.detach(), ins.detach())
 
-    def _run(self, imgs, tgts, bool_masked_pos, valid, seg_type=None, merge_between_batch=-1):
+    def _ensemble(self, i, B, merge_between_batch, prompts_per_query, merge_idx=2):
+        """(groups, members) of the SegGPT prompt ensemble at block i (models_seggpt.py:220-231,:425-429); (0, 0) =
+        none.  By default the ensemble averages over the whole batch, as the reference does.  With prompts_per_query
+        = P the batch holds B / P queries of P prompts each, query-major ([Q][P], so [2][Q][P] before the early
+        merge), and each query averages over its own P members only."""
+        if merge_between_batch < 0 or i < merge_between_batch:
+            return 0, 0
+        P = B if prompts_per_query is None else prompts_per_query
+        if P < 1 or B % P != 0:
+            raise ValueError(f"painter_b200: prompts_per_query {P} does not divide the batch {B}")
+        return (2 * (B // P), P) if merge_idx >= i else (B // P, P)
+
+    def _run(self, imgs, tgts, bool_masked_pos, valid, seg_type=None, merge_between_batch=-1,
+             prompts_per_query=None):
         if not imgs.is_cuda:
             raise RuntimeError("painter_b200 runs on CUDA (sm_90a) only; there is no CPU fallback")
         if valid is None:
@@ -287,13 +300,12 @@ class Painter(nn.Module):
         prec = self.precision
         if prec not in ("auto", "bf16", "fp32"):
             raise ValueError(f"painter_b200: precision must be 'auto', 'bf16' or 'fp32', got {prec!r}")
-        if prec == "fp32" or (prec == "auto" and not torch.is_autocast_enabled("cuda") and
-                              not torch.is_grad_enabled()):
+        from . import accurate
+        if accurate.selected(self):
             if self.training and any(b.drop_prob > 0 for b in self.blocks):
                 raise NotImplementedError("painter_b200: the fp32-accurate mode is an inference mode (call .eval())")
-            from . import accurate
             return accurate.forward(self, imgs.detach(), tgts.detach(), mask_u8, valid,
-                                    self._type_emb(B, seg_type, dev), merge_between_batch)
+                                    self._type_emb(B, seg_type, dev), merge_between_batch, prompts_per_query)
         # gradient arena + per-step token (engine.StageEnv): the arena only when this forward can be followed by a
         # backward that produces parameter gradients.  A fully frozen module (e.g. for prompt tuning) has none, and
         # drops the arena of an earlier training phase.
@@ -321,9 +333,7 @@ class Painter(nn.Module):
             ws = blk.window_size
             if ws > 0 and 112 % ws != 0:
                 raise NotImplementedError(f"painter_b200: window_size {ws} unsupported (must divide 112: 2,4,7,8,14,28)")
-            ens_g, ens_p = 0, 0
-            if merge_between_batch >= 0 and i >= merge_between_batch:
-                ens_g, ens_p = (2, B) if merge_idx >= i else (1, B)
+            ens_g, ens_p = self._ensemble(i, B, merge_between_batch, prompts_per_query, merge_idx)
             da, dm = drops[i]
             prm = stages[f"block{i}"]
             prm["rel_h"] = engine.resize_rel_table(prm["rel_h"], ws if ws > 0 else h)

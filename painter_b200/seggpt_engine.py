@@ -57,7 +57,7 @@ def _graphed(model):
 def stitch_normalize(tops, bottoms, S):
     """tops / bottoms: lists of P device tensors [S, S, 3] (uint8, or fp32 / fp64 in [0, 1]) -> fp32 [P, 3, 2S, S]."""
     P = len(tops)
-    assert P == len(bottoms) and 1 <= P <= 16
+    assert P == len(bottoms) and P >= 1
     dev = tops[0].device
     for t in list(tops) + list(bottoms):
         assert t.is_cuda and t.is_contiguous() and tuple(t.shape) == (S, S, 3) and t.dtype in _DT, (t.shape, t.dtype)
@@ -81,6 +81,89 @@ def seg_postprocess(patch, h, w, p, want_bin=False):
     return out, b
 
 
+def denorm_bottom_batched(patch, B, h, w, p, finish=0, src_stride=1, want_bin=False):
+    """patchified prediction [*, h*w, p*p*3] fp32 -> fp64 [B, h*p/2, w*p, 3]: the bottom half of samples 0, src_stride,
+    2 src_stride, .. de-normalised, then x255 clipped (finish 0), x10000 clipped (1) or left as is (2); optional fp32
+    {0,1} mask [B, h*p/2, w*p] (finish 0 only).  Sample b is what seg_postprocess / denorm_bottom give for it alone."""
+    assert patch.dtype == torch.float32 and patch.is_contiguous() and patch.shape[0] >= (B - 1) * src_stride + 1
+    out = torch.empty((B, h * p // 2, w * p, 3), dtype=torch.float64, device=patch.device)
+    b = torch.empty((B, h * p // 2, w * p), dtype=torch.float32, device=patch.device) if want_bin else None
+    check(lib().pk_denorm_bottom_batched(ctypes.c_void_p(patch.data_ptr()), ctypes.c_void_p(out.data_ptr()),
+                                         ctypes.c_void_p(b.data_ptr()) if b is not None else None, B, src_stride, h,
+                                         w, p, finish, _stream()), "pk_denorm_bottom_batched")
+    return out, b
+
+
+# pk_finish_ragged ops (include/painter_b200.h PK_FIN_*) and their output dtype / elements per pixel
+FIN_BILINEAR_U8, FIN_NEAREST_U8, FIN_DEPTH, FIN_BICUBIC_F64, FIN_NEAREST_BLEND = range(5)
+_FIN_OUT = {FIN_BILINEAR_U8: (torch.uint8, 3), FIN_NEAREST_U8: (torch.uint8, 3), FIN_DEPTH: (torch.int32, 1),
+            FIN_BICUBIC_F64: (torch.float64, 3), FIN_NEAREST_BLEND: (torch.uint8, 3)}
+RAG_FIELDS = 6
+
+
+def ragged_table(op, srcs, sizes, cl_forms=None):
+    """Descriptor table of one pk_finish_ragged launch: image i is finished from source sample srcs[i] to
+    sizes[i] = (OH, OW) with torch-CPU's form cl_forms[i].  Returns (int32 [n, RAG_FIELDS] rows [src, OH, OW, cl_form,
+    offset lo, hi], element offset of every image in the packed output, total elements, largest OH * OW)."""
+    n = len(srcs)
+    if n < 1 or n > 65535 or len(sizes) != n or (cl_forms is not None and len(cl_forms) != n):
+        raise ValueError(f"ragged_table: {n} images (1 .. 65535), {len(sizes)} sizes")
+    per = _FIN_OUT[op][1]
+    tab = np.zeros((n, RAG_FIELDS), dtype=np.int64)
+    offs, off, max_pix = [], 0, 0
+    for i, (s, (oh, ow)) in enumerate(zip(srcs, sizes)):
+        oh, ow, s = int(oh), int(ow), int(s)
+        if s < 0 or oh < 1 or ow < 1 or oh * ow * per >= 2 ** 31:
+            raise ValueError(f"ragged_table: image {i}: source sample {s}, size {oh} x {ow}")
+        tab[i, :4] = (s, oh, ow, int(cl_forms[i]) if cl_forms is not None else 0)
+        tab[i, 4], tab[i, 5] = off & 0xFFFFFFFF, off >> 32
+        offs.append(off)
+        off += oh * ow * per
+        max_pix = max(max_pix, oh * ow)
+    return tab.astype(np.uint32).view(np.int32), offs, off, max_pix
+
+
+def finish_ragged(op, src, table_dev, n, max_pix, total, image=None):
+    """One launch finishing n images from src fp64 [B, SH, SW, 3] into a packed output of `total` elements
+    (table_dev: ragged_table's rows on the device; image: the packed uint8 source images of the blend)."""
+    assert src.dtype == torch.float64 and src.is_contiguous() and src.dim() == 4 and table_dev.dtype == torch.int32
+    assert table_dev.is_contiguous() and table_dev.numel() == n * RAG_FIELDS
+    dst = torch.empty((total,), dtype=_FIN_OUT[op][0], device=src.device)
+    check(lib().pk_finish_ragged(op, ctypes.c_void_p(src.data_ptr()), src.shape[1], src.shape[2],
+                                 ctypes.c_void_p(table_dev.data_ptr()), n, max_pix,
+                                 ctypes.c_void_p(image.data_ptr()) if image is not None else None,
+                                 ctypes.c_void_p(dst.data_ptr()), _stream()), "pk_finish_ragged")
+    return dst
+
+
+_staging = {}
+
+
+def upload(arrays, device):
+    """Copy host arrays to the device in ONE transfer from a reused pinned buffer.  Returns one device tensor per
+    array (same dtype and shape, 16-byte aligned views of one device buffer)."""
+    device = torch.device(device)
+    arrays = [np.ascontiguousarray(a) for a in arrays]
+    offs, n = [], 0
+    for a in arrays:
+        offs.append(n)
+        n += (a.nbytes + 15) // 16 * 16
+    ent = _staging.get(device)
+    if ent is None or ent[0].numel() < n:
+        ent = (torch.empty((max(n, 1),), dtype=torch.uint8, pin_memory=True), torch.cuda.Event())
+        _staging[device] = ent
+    host, done = ent
+    done.synchronize()          # the previous transfer out of the pinned buffer has finished
+    hv = host.numpy()
+    for a, o in zip(arrays, offs):
+        hv[o:o + a.nbytes] = a.reshape(-1).view(np.uint8)
+    dev = torch.empty((max(n, 1),), dtype=torch.uint8, device=device)
+    dev.copy_(host[:max(n, 1)], non_blocking=True)
+    done.record()
+    return [dev[o:o + a.nbytes].view(torch.from_numpy(a[:0].reshape(-1)).dtype).view(a.shape)
+            for a, o in zip(arrays, offs)]
+
+
 def nearest_blend(seg, image_u8):
     """seg fp64 [SH, SW, 3] (0..255), image uint8 [OH, OW, 3] (device) -> uint8 [OH, OW, 3] blended overlay."""
     OH, OW, _ = image_u8.shape
@@ -98,8 +181,9 @@ def _half_mask(model, device):
     return m
 
 
-def _forward(model, x, tgt, device):
-    """The call of seggpt_engine.py:36-47 on device tensors x, tgt [P, 3, 896, 448] fp32; returns patchify(pred)."""
+def _forward(model, x, tgt, device, prompts_per_query=None):
+    """The call of seggpt_engine.py:36-47 on device tensors x, tgt [P, 3, 896, 448] fp32; returns patchify(pred).
+    prompts_per_query: the batch is [Q][P] members of Q queries, each ensembled over its own P prompts."""
     P = x.shape[0]
     key = ("seg_consts", P, str(device), model.seg_type)
     c = model.__dict__.get("_pk_seg_consts")
@@ -109,8 +193,10 @@ def _forward(model, x, tgt, device):
         c = (key, _half_mask(model, device), torch.ones((P, 3, x.shape[2], x.shape[3]), device=device), seg_type)
         model.__dict__["_pk_seg_consts"] = c
     _, mask, valid, seg_type = c
-    feat_ensemble = 0 if P > 1 else -1
-    _, y, _ = _graphed(model)(x, tgt, mask, valid, seg_type, feat_ensemble)
+    group = P if prompts_per_query is None else prompts_per_query
+    feat_ensemble = 0 if group > 1 else -1
+    _, y, _ = _graphed(model)(x, tgt, mask, valid, seg_type, feat_ensemble,
+                              prompts_per_query if feat_ensemble == 0 else None)
     return y
 
 
@@ -154,6 +240,72 @@ def segment(model, device, image_u8, prompts, want_bin=False):
     y = _forward(model, x, t, device)
     p = model.patch_size
     return seg_postprocess(y, 2 * S // p, S // p, p, want_bin=want_bin)
+
+
+@torch.no_grad()
+def segment_batch(model, device, images_u8, prompts, want_bin=False):
+    """segment() of Q queries that share one prompt set, in one forward of Q x P members ([Q][P], each query ensembled
+    over its own P prompts).  images_u8: device uint8 [Q, 448, 448, 3] (or a list of Q such images); prompts as in
+    segment().  Returns (fp64 [Q, 448, 448, 3], optional mask [Q, 448, 448]); entry q equals segment(..., images_u8[q],
+    prompts, want_bin) bit for bit.  A batch smaller than one already captured is padded to it by repeating the last
+    query (its whole prompt group), so a folder runs on one CUDA graph; the padding is dropped."""
+    device = torch.device(device)
+    Q, P = len(images_u8), len(prompts)
+    if Q < 1 or P < 1:
+        raise ValueError(f"segment_batch: {Q} queries, {P} prompts")
+    S = images_u8[0].shape[0]
+    p = model.patch_size
+    g = _graphed(model)
+    Qc = g.captured_batch((Q * P, 3, 2 * S, S), Q * P, P if P > 1 else None) // P
+    qs = [images_u8[q] for q in range(Q)] + [images_u8[Q - 1]] * (Qc - Q)
+    precheck_memory(model, Qc * P, 2 * S, S)
+    x = stitch_normalize([pr[0] for _ in qs for pr in prompts], [q for q in qs for _ in prompts], S)
+    t = stitch_normalize([pr[1] for _ in qs for pr in prompts], [pr[1] for _ in qs for pr in prompts], S)
+    torch.manual_seed(2)      # as segment(): seggpt_engine.py:91, once per forward
+    y = _forward(model, x, t, device, P)
+    # query q is member q * P's bottom half (seggpt_engine.py:48 takes member 0 of its batch)
+    return denorm_bottom_batched(y, Q, 2 * S // p, S // p, p, 0, src_stride=P, want_bin=want_bin)
+
+
+def precheck_memory(model, B, H, W):
+    """Refuse, before any allocation, an fp32-accurate forward of B canvases that cannot fit in the device memory
+    left (accurate.workspace_bytes); the bf16 forward needs far less and is not checked."""
+    from . import accurate
+    if not accurate.selected(model):
+        return
+    need = accurate.workspace_bytes(model, B, H, W)
+    free, _ = torch.cuda.mem_get_info()
+    free += torch.cuda.memory_reserved() - torch.cuda.memory_allocated()
+    if need > free:
+        per = accurate.workspace_bytes(model, 1, H, W)
+        raise RuntimeError(f"painter_b200: an fp32-accurate forward of {B} canvases of {H} x {W} needs about "
+                           f"{need / 2**30:.1f} GiB and {free / 2**30:.1f} GiB is free; use a batch of at most "
+                           f"{max(1, int(free // per))} canvases, or model.precision = 'bf16'")
+
+
+def inference_images(model, device, img_paths, img2_paths, tgt2_paths, out_paths, batch_size=8):
+    """inference_image() over a folder of queries sharing one prompt set, batch_size queries per forward: writes the
+    same PNG files as one inference_image call per query.  Per batch: one upload (the resized queries, the source
+    images and the blend's descriptor table), one forward, one ragged blend launch, one download."""
+    from PIL import Image
+    device = torch.device(device)
+    if len(img_paths) != len(out_paths) or batch_size < 1:
+        raise ValueError("inference_images: one output path per query image, batch_size >= 1")
+    res, hres = 448, 448
+    prompts = [_load_prompt(a, b, res, hres, device) for a, b in zip(img2_paths, tgt2_paths)]
+    for b0 in range(0, len(img_paths), batch_size):
+        images = [Image.open(pth).convert("RGB") for pth in img_paths[b0:b0 + batch_size]]
+        srcs = [np.array(im) for im in images]
+        small = np.stack([np.array(im.resize((res, hres))) for im in images])
+        Q = len(images)
+        tab, offs, total, max_pix = ragged_table(FIN_NEAREST_BLEND, range(Q), [a.shape[:2] for a in srcs])
+        flat = np.concatenate([a.reshape(-1) for a in srcs])
+        small_d, flat_d, tab_d = upload([small, flat, tab], device)
+        out, _ = segment_batch(model, device, small_d, prompts)
+        blended = finish_ragged(FIN_NEAREST_BLEND, out, tab_d, Q, max_pix, total, image=flat_d).cpu().numpy()
+        for q in range(Q):
+            h, w = srcs[q].shape[:2]
+            Image.fromarray(blended[offs[q]:offs[q] + h * w * 3].reshape(h, w, 3)).save(out_paths[b0 + q])
 
 
 def inference_image(model, device, img_path, img2_paths, tgt2_paths, out_path):
