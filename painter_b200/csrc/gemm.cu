@@ -7,8 +7,10 @@
 //                                  gives its registers up (setmaxnreg) to the math warpgroups
 //   warpgroups 1-2  math           (wgmma.mma_async 64 x BN x 16 from shared memory, 64 accumulator rows each;
 //                                  one wgmma group stays in flight while the previous ring slot is released),
-//                                  then the fused epilogue: accumulators -> smem staging tile (64 x 64 per
-//                                  warpgroup) -> coalesced epilogue chunks of 32 x 32 per warp
+//                                  then the fused epilogue: bf16 / GELU outputs in registers -> swizzled smem
+//                                  sub-tiles -> asynchronous TMA stores (gemm_tma_epilogue_tile); the other kinds
+//                                  accumulators -> smem staging tile (64 x 64 per warpgroup) -> coalesced epilogue
+//                                  chunks of 32 x 32 per warp
 // The producer runs up to `stages` K-blocks ahead, so the next tile's operands stream in during an epilogue.
 // Operands may be K-major (row-major [rows,K]) or MN-major (row-major [K,rows]); the latter is what the backward
 // GEMMs (dgrad: B = W[out,in]; wgrad: A = dY[tokens,out], B = X[tokens,in]) need, so no transposed copies of weights
@@ -41,21 +43,86 @@ __device__ __forceinline__ void gemm_kblock(float (&acc)[BN / 2], uint32_t a_add
   wgmma_commit();
 }
 
+// Epilogue of the TMA-store kinds (bf16, GELU) for the 64 accumulator rows of one math warpgroup: alpha and bias on
+// the fragments in registers, each 64-column sub-tile written in the output's 128B-swizzled layout into one of the
+// warpgroup's two staging slots and stored by one thread with cp.async.bulk.tensor.  The warpgroup does not wait for
+// the stores: a slot is only waited on (wait_group.read) when it is about to be rewritten, two sub-tiles later.
+// Every element goes through the same expressions as the staged epilogue (gemm_epilogue_chunk), so the results are
+// bit-identical to it.
+template <int KIND, int BN>
+__device__ __forceinline__ void gemm_tma_epilogue_tile(const GemmArgs& g, const CUtensorMap* tmC,
+                                                       const CUtensorMap* tmC2, const float (&acc)[BN / 2],
+                                                       uint32_t stg_wg, uint32_t& slot, int m_blk, int n_blk, int cw,
+                                                       int wl, int lane) {
+  constexpr uint32_t SLOT = gemm_slot_bytes(KIND);
+  const bool issuer = (threadIdx.x & 127) == 0;
+  const int r0 = 16 * wl + (lane >> 2);   // fragment rows r0 and r0 + 8; both have (row % 8) = lane / 4
+  const uint32_t sw = static_cast<uint32_t>(lane >> 2);
+  const uint32_t off0 = r0 * 128u + 4u * (lane & 3), off1 = off0 + 8u * 128u;
+  const float sc = g.epi.alpha;
+  const float bsc = 1.0f;
+  const float* bias = g.epi.bias;
+#pragma unroll
+  for (int j = 0; j < BN / 64; ++j) {
+    if (issuer) tma_store_wait_read<1>();   // the store that last read this slot (two sub-tiles ago) is done
+    named_bar_sync(1 + cw, 128);
+    const uint32_t buf = stg_wg + slot * SLOT;
+    const int col0 = n_blk * BN + 64 * j;
+#pragma unroll
+    for (int n8 = 0; n8 < 8; ++n8) {
+      const int i = 4 * (8 * j + n8);   // acc[i], acc[i + 1]: row r0; acc[i + 2], acc[i + 3]: row r0 + 8
+      float v[4];
+      if (bias != nullptr) {
+        const float2 b = __ldg(reinterpret_cast<const float2*>(bias + col0 + 8 * n8 + 2 * (lane & 3)));
+        v[0] = fmaf(acc[i], sc, b.x * bsc);
+        v[1] = fmaf(acc[i + 1], sc, b.y * bsc);
+        v[2] = fmaf(acc[i + 2], sc, b.x * bsc);
+        v[3] = fmaf(acc[i + 3], sc, b.y * bsc);
+      } else {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) v[q] = acc[i + q] * sc;
+      }
+      const uint32_t chunk = ((static_cast<uint32_t>(n8) ^ sw) << 4);
+      const uint32_t z0 = pack_bf16x2(v[0], v[1]), z1 = pack_bf16x2(v[2], v[3]);
+      st_shared_u32(buf + off0 + chunk, z0);
+      st_shared_u32(buf + off1 + chunk, z1);
+      if constexpr (KIND == PK_EPI_GELU) {
+        float h[4];
+        gelu_fast_pair(__uint_as_float(z0 << 16), __uint_as_float(z0 & 0xFFFF0000u), h[0], h[1]);
+        gelu_fast_pair(__uint_as_float(z1 << 16), __uint_as_float(z1 & 0xFFFF0000u), h[2], h[3]);
+        st_shared_u32(buf + GEMM_SUB_BYTES + off0 + chunk, pack_bf16x2(h[0], h[1]));
+        st_shared_u32(buf + GEMM_SUB_BYTES + off1 + chunk, pack_bf16x2(h[2], h[3]));
+      }
+    }
+    fence_proxy_async_smem();   // the generic-proxy writes above become visible to the bulk copy
+    named_bar_sync(1 + cw, 128);
+    if (issuer) {
+      const int row0 = m_blk * GEMM_BM + 64 * cw;   // rows past M are clipped by the tensor map
+      tma_store_2d(tmC, buf, col0, row0);
+      if constexpr (KIND == PK_EPI_GELU) tma_store_2d(tmC2, buf + GEMM_SUB_BYTES, col0, row0);
+      tma_store_commit();
+    }
+    slot ^= 1u;
+  }
+}
+
 template <int KIND, int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                 const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmC2,
                  const GemmArgs g) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_base = smem_u32(smem_raw);
   const uint32_t base = (raw_base + 1023u) & ~1023u;
   uint8_t* smem_gen = smem_raw + (base - raw_base);
 
+  constexpr bool TMA_EPI = gemm_tma_epilogue(KIND);
   constexpr uint32_t B_BYTES = static_cast<uint32_t>(BN) * 128u;
   const int stages = g.stages;
   const uint32_t sA = base;
   const uint32_t sB = base + stages * GEMM_A_BYTES;
-  const uint32_t sStg = sB + stages * B_BYTES;
-  const uint32_t bar_base = sStg + GEMM_STG_BYTES;
+  const uint32_t sStg = sB + stages * B_BYTES;   // 1024-aligned (swizzled TMA boxes)
+  const uint32_t bar_base = sStg + gemm_stg_bytes(KIND);
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (stages + s); };
 
@@ -68,6 +135,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    if constexpr (TMA_EPI) tma_prefetch_desc(&tmC);
+    if constexpr (KIND == PK_EPI_GELU) tma_prefetch_desc(&tmC2);
     for (int s = 0; s < stages; ++s) {
       mbar_init(full_bar(s), 1);
       mbar_init(empty_bar(s), 256);   // every math thread releases the slot after its wgmma retired
@@ -143,6 +212,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int wl = warp & 3;              // warp within the warpgroup
   float* stg = reinterpret_cast<float*>(smem_gen + (sStg - base)) + cw * 64 * STG_LD;
   const int frag_r = 16 * wl + (lane >> 2), frag_c = 2 * (lane & 3);
+  const uint32_t stg_wg = sStg + cw * 2u * gemm_slot_bytes(KIND);   // TMA-store kinds: this warpgroup's two slots
+  uint32_t slot = 0;
   uint32_t s = 0, ph = 0;
   float acc[BN / 2];
   while (sch.next(mn, kb0, kb1)) {
@@ -175,6 +246,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     mbar_arrive(empty_bar(prev));
 
     // --------------------------------- epilogue ---------------------------------
+    if constexpr (TMA_EPI) {
+      gemm_tma_epilogue_tile<KIND, BN>(g, &tmC, &tmC2, acc, stg_wg, slot, m_blk, n_blk, cw, wl, lane);
+      continue;
+    }
 #pragma unroll
     for (int c0 = 0; c0 < BN; c0 += 64) {
       named_bar_sync(1 + cw, 128);     // the previous chunk's readers are done with the staging tile
@@ -230,13 +305,18 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       }
     }
   }
+  // the bulk stores read shared memory and must have written their results before the CTA exits: shared memory is
+  // released then, and a dependent launch (PDL) only waits for this grid to complete
+  if constexpr (TMA_EPI) {
+    if ((threadIdx.x & 127) == 0) tma_store_wait_all();
+  }
 }
 
 int g_force_bn = 0;
 int g_force_splits = 0;
 
 static size_t gemm_smem_bytes(const GemmArgs& g) {
-  return 1024 + static_cast<size_t>(g.stages) * (GEMM_A_BYTES + g.BN * 128) + GEMM_STG_BYTES + 256;
+  return 1024 + static_cast<size_t>(g.stages) * (GEMM_A_BYTES + g.BN * 128) + gemm_stg_bytes(g.epi.kind) + 256;
 }
 
 // persistent CTAs a call runs: one per stream-K range, otherwise one per work item up to the SM count
@@ -248,9 +328,14 @@ static int gemm_workers(const GemmArgs& g) {
   return items < sm_count() ? static_cast<int>(items) : sm_count();
 }
 
+// The output tensor maps of the TMA-store epilogues (tmC: out, tmC2: GELU's out2); other kinds pass unused maps.
+struct GemmOutMaps {
+  CUtensorMap c, c2;
+};
+
 template <int KK, int BN>
-static cudaError_t launch_gemm_kernel(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmArgs& g,
-                                      cudaStream_t st) {
+static cudaError_t launch_gemm_kernel(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmOutMaps& tmo,
+                                      const GemmArgs& g, cudaStream_t st) {
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(gemm_bf16_kernel<KK, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -259,30 +344,30 @@ static cudaError_t launch_gemm_kernel(const CUtensorMap& tmA, const CUtensorMap&
     attr_set = true;
   }
   return launch_pdl(gemm_bf16_kernel<KK, BN>, dim3(gemm_workers(g)), dim3(GEMM_THREADS), gemm_smem_bytes(g), st,
-                    tmA, tmB, g);
+                    tmA, tmB, tmo.c, tmo.c2, g);
 }
 
 template <int KK>
-static cudaError_t launch_gemm_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmArgs& g,
-                                  cudaStream_t st) {
-  if (g.BN == 256) return launch_gemm_kernel<KK, 256>(tmA, tmB, g, st);
-  if (g.BN == 128) return launch_gemm_kernel<KK, 128>(tmA, tmB, g, st);
-  return launch_gemm_kernel<KK, 64>(tmA, tmB, g, st);
+static cudaError_t launch_gemm_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmOutMaps& tmo,
+                                  const GemmArgs& g, cudaStream_t st) {
+  if (g.BN == 256) return launch_gemm_kernel<KK, 256>(tmA, tmB, tmo, g, st);
+  if (g.BN == 128) return launch_gemm_kernel<KK, 128>(tmA, tmB, tmo, g, st);
+  return launch_gemm_kernel<KK, 64>(tmA, tmB, tmo, g, st);
 }
 
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmArgs& g, cudaStream_t st,
-                       const char* who) {
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmOutMaps& tmo, GemmArgs& g,
+                       cudaStream_t st, const char* who) {
   PK_CHECK(gemm_smem_bytes(g) <= 227 * 1024 && g.stages >= 2, "%s: BN=%d does not fit shared memory", who, g.BN);
   cudaError_t e = cudaSuccess;
   switch (g.epi.kind) {
-    case PK_EPI_BF16: e = launch_gemm_bn<PK_EPI_BF16>(tmA, tmB, g, st); break;
-    case PK_EPI_F32: e = launch_gemm_bn<PK_EPI_F32>(tmA, tmB, g, st); break;
-    case PK_EPI_GELU: e = launch_gemm_bn<PK_EPI_GELU>(tmA, tmB, g, st); break;
-    case PK_EPI_RESID: e = launch_gemm_bn<PK_EPI_RESID>(tmA, tmB, g, st); break;
-    case PK_EPI_DGELU: e = launch_gemm_bn<PK_EPI_DGELU>(tmA, tmB, g, st); break;
-    case PK_EPI_PIXSHUF: e = launch_gemm_bn<PK_EPI_PIXSHUF>(tmA, tmB, g, st); break;
-    case EPI_HEAD: e = launch_gemm_kernel<EPI_HEAD, 64>(tmA, tmB, g, st); break;
-    case EPI_UNSHUF: e = launch_gemm_kernel<EPI_UNSHUF, 64>(tmA, tmB, g, st); break;
+    case PK_EPI_BF16: e = launch_gemm_bn<PK_EPI_BF16>(tmA, tmB, tmo, g, st); break;
+    case PK_EPI_F32: e = launch_gemm_bn<PK_EPI_F32>(tmA, tmB, tmo, g, st); break;
+    case PK_EPI_GELU: e = launch_gemm_bn<PK_EPI_GELU>(tmA, tmB, tmo, g, st); break;
+    case PK_EPI_RESID: e = launch_gemm_bn<PK_EPI_RESID>(tmA, tmB, tmo, g, st); break;
+    case PK_EPI_DGELU: e = launch_gemm_bn<PK_EPI_DGELU>(tmA, tmB, tmo, g, st); break;
+    case PK_EPI_PIXSHUF: e = launch_gemm_bn<PK_EPI_PIXSHUF>(tmA, tmB, tmo, g, st); break;
+    case EPI_HEAD: e = launch_gemm_kernel<EPI_HEAD, 64>(tmA, tmB, tmo, g, st); break;
+    case EPI_UNSHUF: e = launch_gemm_kernel<EPI_UNSHUF, 64>(tmA, tmB, tmo, g, st); break;
     default:
       PK_CHECK(false, "%s: bad epilogue kind %d", who, g.epi.kind);
   }
@@ -339,7 +424,7 @@ static void plan_gemm(int M, int N, int K, int transA, int transB, const PkEpilo
   }
   if (g_force_bn > 0 && N % g_force_bn == 0) BN = g_force_bn;
   g.BN = BN;
-  g.stages = gemm_stages_for(GEMM_A_BYTES + BN * 128);
+  g.stages = gemm_stages_for(GEMM_A_BYTES + BN * 128, epi->kind);
   g.num_m_tiles = mt;
   g.num_n_tiles = N / BN;
   const int num_kb = (K + GEMM_BK - 1) / GEMM_BK;
@@ -347,7 +432,7 @@ static void plan_gemm(int M, int N, int K, int transA, int transB, const PkEpilo
   g.kb_per_split = num_kb;
   if (zero_init_f32) {
     // zero-initialised fp32 output (weight gradients): stream-K.  The tiles_mn * num_kb k-block units are cut into
-    // one equal range per CTA; a tile that straddles ranges is finished with fp32 atomics.
+    // consecutive ranges of streamk_units, one per CTA; a tile that straddles ranges is finished with fp32 atomics.
     const int tiles = g.num_m_tiles * g.num_n_tiles;
     const long long units = static_cast<long long>(tiles) * num_kb;
     if (g_force_splits > 0) {
@@ -358,7 +443,22 @@ static void plan_gemm(int M, int N, int K, int transA, int transB, const PkEpilo
     } else if (tiles % sms == 0 || units < 4ll * sms) {
       g.epi.accumulate = 1;   // already balanced (or too small to matter): plain data-parallel tiles
     } else {
-      int per = static_cast<int>((units + sms - 1) / sms);
+      // Range length: a whole number of K-phases (num_kb / q, q <= 8) where that costs at most ~10 % over the equal
+      // cut.  Every range then starts at one of q K-offsets, so the CTAs running together read the same few K-slices
+      // of both operands and share them in L2; with the equal cut the starting K-blocks of the 132 ranges are spread
+      // over all of K and nearly every operand block comes from HBM once per CTA that reads it (fc1 weight gradient
+      // at B = 8: 2 whole tiles per CTA on 128 CTAs instead of 381 of 196 K-blocks each).
+      const int equal = static_cast<int>((units + sms - 1) / sms);
+      int per = equal;
+      for (int q = 1; q <= 8; q *= 2) {
+        if (num_kb % q != 0) continue;
+        const int seg = num_kb / q;
+        const int k = static_cast<int>((units + static_cast<long long>(sms) * seg - 1) / (static_cast<long long>(sms) * seg));
+        if (static_cast<long long>(k) * seg * 10 <= static_cast<long long>(equal) * 11) {
+          per = k * seg;
+          break;
+        }
+      }
       if (per < 4) per = 4;
       g.streamk_units = per;
     }
@@ -453,7 +553,20 @@ extern "C" int pk_gemm_bf16(const void* A, const void* B, int M, int N, int K, i
     strides[0] = static_cast<uint64_t>(ldb) * 2;
     if (!make_tmap_bf16(&tmB, B, 2, dims, strides, box)) return 3;
   }
-  return launch_gemm(tmA, tmB, g, static_cast<cudaStream_t>(stream), "pk_gemm_bf16");
+  GemmOutMaps tmo;
+  memset(&tmo, 0, sizeof(tmo));
+  if (gemm_tma_epilogue(epi->kind)) {
+    // [M, N] bf16 outputs with row stride ldc, stored in 64 x 64 boxes; rows past M are clipped
+    PK_CHECK((reinterpret_cast<uintptr_t>(epi->out) & 15) == 0 &&
+                 (epi->kind != PK_EPI_GELU || (reinterpret_cast<uintptr_t>(epi->out2) & 15) == 0),
+             "pk_gemm_bf16: outputs must be 16-byte aligned");
+    const uint64_t dims[2] = {static_cast<uint64_t>(N), static_cast<uint64_t>(M)};
+    const uint64_t strides[1] = {static_cast<uint64_t>(epi->ldc) * 2};
+    const uint32_t box[2] = {64, 64};
+    if (!make_tmap_bf16(&tmo.c, epi->out, 2, dims, strides, box)) return 3;
+    if (epi->kind == PK_EPI_GELU && !make_tmap_bf16(&tmo.c2, epi->out2, 2, dims, strides, box)) return 3;
+  }
+  return launch_gemm(tmA, tmB, tmo, g, static_cast<cudaStream_t>(stream), "pk_gemm_bf16");
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -468,7 +581,7 @@ static int conv_common(const void* img_nhwc, const void* wmat, int B, int H, int
   g.N = 64;
   g.K = 576;
   g.BN = 64;
-  g.stages = gemm_stages_for(GEMM_A_BYTES + 64 * 128);
+  g.stages = gemm_stages_for(GEMM_A_BYTES + 64 * 128, g.epi.kind);
   g.transA = g.transB = 0;
   g.splits = 1;
   g.kb_per_split = 9;
@@ -486,7 +599,9 @@ static int conv_common(const void* img_nhwc, const void* wmat, int B, int H, int
   uint64_t s2[1] = {576 * 2};
   uint32_t b2[2] = {64, 64};
   if (!make_tmap_bf16(&tmB, wmat, 2, d2, s2, b2)) return 3;
-  return launch_gemm(tmA, tmB, g, static_cast<cudaStream_t>(stream), who);
+  GemmOutMaps tmo;
+  memset(&tmo, 0, sizeof(tmo));
+  return launch_gemm(tmA, tmB, tmo, g, static_cast<cudaStream_t>(stream), who);
 }
 
 extern "C" int pk_decoder_head_fwd(const void* g_nhwc, const void* wmat, const float* head_params,
@@ -540,7 +655,7 @@ extern "C" int pk_conv3x3_wgrad(const void* g_nhwc, const void* dc1_nhwc, float*
   GemmArgs g;
   memset(&g, 0, sizeof(g));
   g.M = 576; g.N = 64; g.K = B * H * W;
-  g.BN = 64; g.stages = gemm_stages_for(GEMM_A_BYTES + 64 * 128);
+  g.BN = 64; g.stages = gemm_stages_for(GEMM_A_BYTES + 64 * 128, PK_EPI_F32);
   g.transA = g.transB = 1;
   g.conv.mode = 2;
   g.conv.H = H; g.conv.W = W; g.conv.TW = TW; g.conv.TH = TH;
@@ -563,5 +678,7 @@ extern "C" int pk_conv3x3_wgrad(const void* g_nhwc, const void* dc1_nhwc, float*
   uint32_t box[4] = {64, static_cast<uint32_t>(TW), static_cast<uint32_t>(TH), 1};
   if (!make_tmap_bf16(&tmA, g_nhwc, 4, dims, strides, box)) return 3;
   if (!make_tmap_bf16(&tmB, dc1_nhwc, 4, dims, strides, box)) return 3;
-  return launch_gemm(tmA, tmB, g, static_cast<cudaStream_t>(stream), "pk_conv3x3_wgrad");
+  GemmOutMaps tmo;
+  memset(&tmo, 0, sizeof(tmo));
+  return launch_gemm(tmA, tmB, tmo, g, static_cast<cudaStream_t>(stream), "pk_conv3x3_wgrad");
 }

@@ -40,9 +40,20 @@ struct HeadArgs {
   int slot;                 // which copy of the head parameters in constant memory this launch reads
 };
 
-// operand ring depth that fits beside the two epilogue staging tiles
-__host__ inline int gemm_stages_for(int stage_bytes) {
-  const int budget = 227 * 1024 - 1024 - 256 - GEMM_STG_BYTES;
+// Epilogues whose results leave through TMA stores (gemm.cu): every math warpgroup applies the epilogue to its
+// accumulator fragments and writes 64-column bf16 sub-tiles (64 rows x 128 B, 128B-swizzled: one TMA box) into one of
+// two staging slots; a slot holds one sub-tile per output (GELU: z and gelu(z)).
+__host__ __device__ constexpr bool gemm_tma_epilogue(int kind) { return kind == PK_EPI_BF16 || kind == PK_EPI_GELU; }
+constexpr int GEMM_SUB_BYTES = 64 * 128;   // one 64 x 64 bf16 sub-tile
+__host__ __device__ constexpr int gemm_slot_bytes(int kind) { return (kind == PK_EPI_GELU ? 2 : 1) * GEMM_SUB_BYTES; }
+// staging bytes of a kind: 2 math warpgroups x 2 slots, or the fp32 staging tiles of the other epilogues
+__host__ __device__ constexpr int gemm_stg_bytes(int kind) {
+  return gemm_tma_epilogue(kind) ? 2 * 2 * gemm_slot_bytes(kind) : GEMM_STG_BYTES;
+}
+
+// operand ring depth that fits beside the epilogue staging of `kind`
+__host__ inline int gemm_stages_for(int stage_bytes, int kind) {
+  const int budget = 227 * 1024 - 1024 - 256 - gemm_stg_bytes(kind);
   int st = budget / stage_bytes;
   return st > 8 ? 8 : st;
 }
@@ -65,8 +76,8 @@ struct GemmArgs {
 
 // Work iterator shared by the producer and math roles of the persistent kernel: each role walks the same sequence
 // of (output tile, k-block range) items.  Classic mode: item = (tile, split) strided over the CTAs; stream-K mode:
-// the tiles_mn * num_kb k-block units are cut into equal consecutive ranges, one per CTA, so the machine is full
-// whatever the tile count (weight-gradient GEMMs have 32..128 tiles for 132 SMs).
+// the tiles_mn * num_kb k-block units are cut into consecutive ranges of equal length, one per CTA, so the machine
+// is full whatever the tile count (weight-gradient GEMMs have 32..256 tiles for 132 SMs).
 struct GemmSched {
   int tiles_mn, num_kb, kbps, total, ncl, cur, end;
   bool sk;
