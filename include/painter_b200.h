@@ -386,6 +386,44 @@ int pk_aug_normalize(const uint8_t* slots, int B, int P, int S, float* img, floa
 int pk_aug_second_crop(const float* img, const float* tgt, const int* jobs, int B, int OH, int OW, float* wts,
                        int* bounds, float* tmp, float* img_out, float* tgt_out, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Task metrics (csrc/metrics.cu, painter_b200/task_metrics.py): the scores of the reference's evaluators from the eval
+ * outputs on the device, with no host round trip.  A launch covers a batch of images described by an int64 device
+ * table, one row of PK_METRIC_FIELDS per image: [pred, pred_staged, gt offset, H, W].  pred is the prediction's device
+ * address, or its byte offset from `base` when pred_staged != 0; the ground truth is at base + gt offset (base: the
+ * caller's upload buffer).
+ *  pk_palette_classes     out uint8 [npix] = argmin_k dist(segm[i], palette[k]), the first minimum, with the distance of
+ *                         SemSegEvaluatorCustom.post_process_segm_output (Painter/eval/ade20k_semantic/
+ *                         ADE20kSemSegEvaluatorCustom.py:114-141): PK_DIST_ABS sum |c - P|, PK_DIST_SQUARE sum (c - P)^2,
+ *                         PK_DIST_MEAN sum (|c - P| + (c - P)^2) / 2.  segm uint8 [npix, 3], palette uint8 [K, 3],
+ *                         1 <= K <= 200.
+ *  pk_semseg_confusion    conf int64 [(K+1) * (K+1)] += the counts of cell (K + 1) * class(pred) + gt over every pixel
+ *                         of the n images (pred uint8 [H, W, 3], gt uint8 [H, W]; gt == ignore_label counts as K), as
+ *                         the evaluator's np.bincount (:96-101).  Labels >= K other than ignore_label are the caller's
+ *                         to refuse.  max_pix >= every H * W sizes the grid.
+ *  pk_depth_errors        out fp64 [n, 9] = {d1, d2, d3, AbsRel, SqRel, RMSE, RMSElog, SILog, log10} of Painter/eval/
+ *                         nyuv2_depth/eval_with_pngs.py (pred int32 [H, W] / 1000 clamped into [min_depth, max_depth],
+ *                         gt uint16 [H, W] / 1000, pixels min_depth < gt < max_depth, Eigen crop rows 45:471, columns
+ *                         41:601 when eigen_crop != 0).  One CTA per image.
+ *  pk_restoration_scores  psnr, ssim fp64 [n]: skimage 0.19 peak_signal_noise_ratio(x, y) and structural_similarity(
+ *                         x, y, multichannel=True) as Painter/eval/lol/painter_inference_lol.py calls them, x =
+ *                         clip(pred, 0, 1) (pred fp64 [H, W, 3]), y = gt / 255. (gt uint8 [H, W, 3]); c1, c2 the SSIM
+ *                         constants.  Every image is at least 7 x 7; max_h, max_w bound every H, W.  counters_zeroed
+ *                         uint32 [n] (zero on entry); partials fp64 [n * pk_restoration_ws_doubles(max_h, max_w)].
+ * All results are bitwise reproducible (integer sums, or fp64 sums in a fixed order).                             */
+enum { PK_METRIC_FIELDS = 5 };
+enum { PK_DIST_ABS = 0, PK_DIST_SQUARE = 1, PK_DIST_MEAN = 2 };
+int pk_palette_classes(const uint8_t* segm, long long npix, const uint8_t* palette, int K, int dist_type, uint8_t* out,
+                       void* stream);
+int pk_semseg_confusion(const long long* items, const void* base, int n, long long max_pix, const uint8_t* palette,
+                        int K, int dist_type, int ignore_label, long long* conf, void* stream);
+int pk_depth_errors(const long long* items, const void* base, int n, float min_depth, float max_depth, int eigen_crop,
+                    double* out, void* stream);
+long long pk_restoration_ws_doubles(int max_h, int max_w);
+int pk_restoration_scores(const long long* items, const void* base, int n, int max_h, int max_w,
+                          unsigned* counters_zeroed, double* partials, double c1, double c2, double* psnr, double* ssim,
+                          void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -7,9 +7,9 @@ executed as the live oracle / reference arm:
 
 The reference is pure Python with no setup.py, so `pip install --target oracle/_ref <reference>` has nothing to
 build (recorded in DESIGN.md); this script is the install step.  Only the files of the hot path, its two engines,
-the runtime utilities they import, the task eval scripts (for their run_one_image), the data pipeline used by the
-parity tests and the SegGPT example images are copied, byte for byte; nothing under oracle/_ref is tracked by git or
-imported by the product path.
+the runtime utilities they import, the task eval scripts (for their run_one_image), the task evaluators and palette
+generators (for the metric parity tests), the data pipeline used by the parity tests and the SegGPT example images are
+copied, byte for byte; nothing under oracle/_ref is tracked by git or imported by the product path.
 """
 import filecmp
 import os
@@ -36,6 +36,12 @@ FILES = [
     "Painter/eval/sidd/painter_inference_sidd.py",
     "Painter/eval/lol/painter_inference_lol.py",
     "Painter/eval/derain/painter_inference_derain.py",
+    "Painter/eval/ade20k_semantic/ADE20kSemSegEvaluatorCustom.py",
+    "Painter/eval/coco_panoptic/COCOPanoSemSegEvaluatorCustom.py",
+    "Painter/eval/nyuv2_depth/eval_with_pngs.py",
+    "Painter/data/ade20k/gen_color_ade20k_sem.py",
+    "Painter/data/coco_semseg/gen_color_coco_panoptic_segm.py",
+    "Painter/data/panoptic_coco_categories.json",
     "SegGPT/SegGPT_inference/models_seggpt.py",
     "SegGPT/SegGPT_inference/seggpt_engine.py",
     "SegGPT/SegGPT_inference/seggpt_inference.py",
