@@ -424,6 +424,75 @@ int pk_restoration_scores(const long long* items, const void* base, int n, int m
                           unsigned* counters_zeroed, double* partials, double c1, double c2, double* psnr, double* ssim,
                           void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * COCO panoptic post-processing (csrc/panoptic.cu, painter_b200/panoptic.py): Painter/eval/coco_panoptic's instance
+ * decoding, matrix NMS, class vote and panoptic merge on the device.  A launch covers a batch of n images described by
+ * an int64 device table, one row of PK_PANO_FIELDS per image: [pixels, staged, H, W].  pixels is the uint8 [H, W, 3]
+ * image's device address, or its byte offset from `base` when staged == 1.  Mask tables (pack_masks, unpack outputs)
+ * hold [bool / int32 [.., H, W] device address, rows, H, W].  Per image, `ncap` rows of `words` uint32 (a multiple of
+ * 32) hold the bit rows of its masks (bit p of row i: pixel p in mask i).
+ *  pk_pano_candidates     area int32 [n, T, P], sumfx int64 [n, T, P] (zeroed by the caller) += the pixel count and the
+ *                         2^-25 fixed-point sum of dist = fp32(L1) * fp32(1/3) of candidate (t, c) = {p : L1(p, P_c) <
+ *                         bounds[t]} (COCOCAInstSegEvaluatorCustom.py:283-299, the (num_color, h, w) dist / mask
+ *                         tensors); P <= PK_PANO_MAX_PALETTE colours, T <= PK_PANO_MAX_THR thresholds.
+ *  pk_pano_select         the non-empty candidates sorted stably by (maskness, t * P + c), the first `keep`: count
+ *                         int32 [n], cand int32 [n, ncap], scores fp32 [n, ncap] = 1 - m / max(max m, 1) (:312-325).
+ *                         ws: pk_pano_select_ws_bytes(n, T * P) bytes.
+ *  pk_pano_pack_candidates  bits of the kept candidates cand[i], i < count.
+ *  pk_pano_pack_masks     bits of explicit bool masks (one table row per image); aux int64 [n, 2] rows [fp32 scores
+ *                         address, int64 classes address or 0] gathered into scores fp32 / classes int64 [n, ncap].
+ *  pk_pano_gram           gram int32 [n, ncap, ncap]: popc(row_i & row_j) on every 128 x 128 tile on or above the
+ *                         diagonal with a row below count (util/matrix_nms.py:64-67 inter_matrix); ncap a multiple
+ *                         of 128.
+ *  pk_pano_nms            mask_matrix_nms (util/matrix_nms.py:53-121, gaussian kernel, filter_thr -1, nms_pre -1):
+ *                         rows int32 [n, max_num] (input indices), out_scores fp32 [n, max_num], out_count [n],
+ *                         out_labels int64 [n, max_num] or null (labels[row], 1 without labels).  labels
+ *                         int64 [n, ncap] or null (class-agnostic); gram null: no decay, the stable descending order
+ *                         only.  empty_one: an image without candidates gets one row -1 with score 0 (:301-310).
+ *                         ws: 4 * n * ncap int32.
+ *  pk_pano_unpack         bool masks out[i] = row rows[img * rows_ld + i] (zeros for -1).
+ *  pk_pano_minmax         post_process_segm_output_by_minmax (:172-250): pred int16 [n, max_pix] = the first nearest
+ *                         of the P colours and black (index P); cnt, sum [n, P + 1] (zeroed); cols / scores / classes
+ *                         [n, P + 1] and count [n]: the colours present in index order.
+ *  pk_pano_minmax_masks   bool masks out[i] = (pred == cols[img * P1 + i]).
+ *  pk_pano_vote           classes int64 [n, ncap] = argmax_k sum over the mask of 1 - d_k / max d (k < 80, d the L1
+ *                         distance to semantic colour k; COCOPanoEvaluatorCustom.py:259-276); dmax_zeroed int32 [n].
+ *  pk_pano_merge          combine_semantic_and_instance_outputs_custom (COCOPanoEvaluatorCustom.py:47-134): int32
+ *                         maps (zeroed) from the instances' bits / scores / classes and the semantic argmin map (labels
+ *                         uint8 [n, max_pix] workspace; 80 <= K <= 200); segs int64 [n, max_seg, 4] = {instance or -1,
+ *                         category, area, fp32 score bits}, nseg int32 [n].
+ * All results are bitwise reproducible (integer sums and counts, stable orders on explicit keys).                  */
+enum { PK_PANO_FIELDS = 4, PK_PANO_MAX_PALETTE = 6400, PK_PANO_MAX_THR = 4 };
+int pk_pano_candidates(const long long* items, const void* base, int n, long long max_pix, const uint8_t* palette,
+                       int P, const int* bounds, int T, int* area, long long* sumfx, void* stream);
+long long pk_pano_select_ws_bytes(int n, int NC);
+int pk_pano_select(const int* area, const long long* sumfx, int n, int NC, int keep, int ncap, void* ws,
+                   long long ws_bytes, int* count, int* cand, float* scores, void* stream);
+int pk_pano_pack_candidates(const long long* items, const void* base, int n, const uint8_t* palette, int P,
+                            const int* bounds, int T, const int* cand, const int* count, int ncap, int words,
+                            uint32_t* bits, void* stream);
+int pk_pano_pack_masks(const long long* items, int n, int max_rows, int ncap, int words, uint32_t* bits,
+                       const long long* aux, float* scores, long long* classes, void* stream);
+int pk_pano_gram(const uint32_t* bits, int n, int ncap, int words, const int* count, int* gram, void* stream);
+int pk_pano_nms(const int* gram, const long long* labels, const float* scores, const int* count, int n, int ncap,
+                float sigma, int max_num, int empty_one, int* ws, int* rows, float* out_scores, int* out_count,
+                long long* out_labels, void* stream);
+int pk_pano_unpack(const uint32_t* bits, int n, int ncap, int words, const int* rows, int rows_ld, int max_rows,
+                   long long max_pix, const long long* outs, void* stream);
+int pk_pano_minmax(const long long* items, const void* base, int n, long long max_pix, const uint8_t* palette, int P,
+                   short* pred, int* cnt, long long* sum, int* cols, float* scores, long long* classes, int* count,
+                   void* stream);
+int pk_pano_minmax_masks(const short* pred, int n, long long max_pix, const int* cols, int P1, int max_rows,
+                         const long long* outs, void* stream);
+int pk_pano_vote(const long long* items, const void* base, int n, long long max_pix, const uint8_t* palette,
+                 const uint32_t* bits, int ncap, int words, const int* count, int max_rows, int* dmax_zeroed,
+                 long long* classes, void* stream);
+long long pk_pano_merge_smem(int words, int ncap);
+int pk_pano_merge(const long long* sem_items, const void* base, const long long* maps, int n, long long max_pix,
+                  const uint8_t* palette, int K, uint8_t* labels, const uint32_t* bits, int ncap, int words,
+                  const float* scores, const long long* classes, const int* count, double overlap, double stuff_area,
+                  double score_thresh, int max_seg, long long* segs, int* nseg, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -38,6 +38,9 @@ FILES = [
     "Painter/eval/derain/painter_inference_derain.py",
     "Painter/eval/ade20k_semantic/ADE20kSemSegEvaluatorCustom.py",
     "Painter/eval/coco_panoptic/COCOPanoSemSegEvaluatorCustom.py",
+    "Painter/eval/coco_panoptic/COCOCAInstSegEvaluatorCustom.py",
+    "Painter/eval/coco_panoptic/COCOInstSegEvaluatorCustom.py",
+    "Painter/eval/coco_panoptic/COCOPanoEvaluatorCustom.py",
     "Painter/eval/nyuv2_depth/eval_with_pngs.py",
     "Painter/data/ade20k/gen_color_ade20k_sem.py",
     "Painter/data/coco_semseg/gen_color_coco_panoptic_segm.py",
