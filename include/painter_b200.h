@@ -493,6 +493,32 @@ int pk_pano_merge(const long long* sem_items, const void* base, const long long*
                   const float* scores, const long long* classes, const int* count, double overlap, double stuff_area,
                   double score_thresh, int max_seg, long long* segs, int* nseg, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * COCO pose post-processing (csrc/pose.cu, painter_b200/pose.py): Painter/eval/mmpose_custom's heatmap decoding, flip
+ * averaging, keypoint decoding, rescoring and OKS NMS on the device.
+ *  pk_pose_decode   out fp32 [n, 17, 3] = (x, y, maxval) of forward_pseudo_test + the head's decode (model/top_down.py
+ *                   :163-258; flip_test iff flipped images are given, shift_heatmap, post_process 'default', no UDP).
+ *                   items int64 [n, PK_POSE_FIELDS] rows [pred, pred staged, flipped, flipped staged]: a uint8
+ *                   [H, W, 3] image's device address, or its byte offset from `base` when staged == 1; flipped staged
+ *                   == 2: no flipped image (all rows alike).  palette: host uint8 [18, 2] (G, B); swap: host int32 [17]
+ *                   (flip_back's channel swap); cs fp32 [n, 4] rows (center x, y, scale x, y); keys_zeroed u64
+ *                   [n, 17] and done_zeroed u32 [n] zeroed workspace.  H, W >= 3.
+ *  pk_pose_nms      the rescoring and oks_nms of data/topdown_coco_dataset.py:266-297 for n_img images, one CTA each:
+ *                   images int32 [n_img, 2] rows (start, count) into pos int32 (box rows of kpts fp32 [N, 51],
+ *                   box_scores fp32 [N], areas fp32 [N]), each image's boxes in bbox_id order, count <= 1024.  vars:
+ *                   host fp64 [17] = (2 sigma)^2.  Order: score descending, ties the later box first.  rows int32
+ *                   [sum count, PK_POSE_ROW] from each image's start, in keep order: (pos, fp32 score bits, 51 fp32
+ *                   keypoint bits); counts int32 [n_img] kept.  Shared memory: pk_pose_nms_smem(max count).
+ * Results are bitwise reproducible (key maxima, explicitly rounded arithmetic, explicit orders).                     */
+enum { PK_POSE_FIELDS = 4, PK_POSE_JOINTS = 17, PK_POSE_PALETTE = 18, PK_POSE_MAX_BOXES = 1024, PK_POSE_ROW = 53 };
+int pk_pose_decode(const long long* items, const void* base, int n, int H, int W, const uint8_t* palette,
+                   const int* swap, const float* cs, unsigned long long* keys_zeroed, unsigned* done_zeroed,
+                   float* out, void* stream);
+long long pk_pose_nms_smem(int max_count);
+int pk_pose_nms(const int* images, int n_img, int max_count, const int* pos, const float* kpts,
+                const float* box_scores, const float* areas, const double* vars, float vis_thr, float oks_thr,
+                int* rows, int* counts, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

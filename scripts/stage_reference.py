@@ -8,7 +8,8 @@ executed as the live oracle / reference arm:
 The reference is pure Python with no setup.py, so `pip install --target oracle/_ref <reference>` has nothing to
 build (recorded in DESIGN.md); this script is the install step.  Only the files of the hot path, its two engines,
 the runtime utilities they import, the task eval scripts (for their run_one_image), the task evaluators and palette
-generators (for the metric parity tests), the data pipeline used by the parity tests and the SegGPT example images are
+generators (for the metric parity tests), the pose model, dataset, colour and keypoint definitions of
+eval/mmpose_custom (for the pose parity tests), the data pipeline used by the parity tests and the SegGPT example images are
 copied, byte for byte; nothing under oracle/_ref is tracked by git or imported by the product path.
 """
 import filecmp
@@ -41,6 +42,10 @@ FILES = [
     "Painter/eval/coco_panoptic/COCOCAInstSegEvaluatorCustom.py",
     "Painter/eval/coco_panoptic/COCOInstSegEvaluatorCustom.py",
     "Painter/eval/coco_panoptic/COCOPanoEvaluatorCustom.py",
+    "Painter/eval/mmpose_custom/model/top_down.py",
+    "Painter/eval/mmpose_custom/data/topdown_coco_dataset.py",
+    "Painter/eval/mmpose_custom/data/pipelines/custom_transform.py",
+    "Painter/eval/mmpose_custom/configs/_base_/coco.py",
     "Painter/eval/nyuv2_depth/eval_with_pngs.py",
     "Painter/data/ade20k/gen_color_ade20k_sem.py",
     "Painter/data/coco_semseg/gen_color_coco_panoptic_segm.py",
