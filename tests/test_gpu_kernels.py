@@ -284,10 +284,12 @@ def test_attention_fwd_bwd_vs_reference_math(B, heads, h, w):
     out2, lse2, rel = ops.attn_fwd(qkv, th, tw, B, heads, h, w, save_rel=True)
     assert torch.equal(out2, out) and torch.equal(lse2, lse)
     dqkv2, dTh2, dTw2 = ops.attn_bwd(qkv, out2, dout, lse2, th, tw, B, heads, h, w, rel=rel)
+    # the forward stores the bias rows the recomputing pair's bias-row kernel computes with the same instructions, and
+    # the dQ / dK/dV kernels read them the same way: the two pairs agree bit for bit
+    assert torch.equal(dqkv2, dqkv), "saved vs recomputed"
     d2 = dqkv2.float().reshape(B * N, 3, C)
     for i in range(3):
         assert relmax(d2[:, i], g[:, i]) < 2e-2, "saved " + "qkv"[i]
-        assert relmax(d2[:, i], d[:, i]) < 2e-3, "saved vs recomputed " + "qkv"[i]
     assert relmax(dTh2, t32.grad[:2 * h - 1]) < 2e-2 and relmax(dTw2, w32.grad[:2 * w - 1]) < 2e-2
 
 
