@@ -425,6 +425,32 @@ int pk_restoration_scores(const long long* items, const void* base, int n, int m
                           void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * MATLAB-scored restoration benchmarks (csrc/restoration_matlab.cu, painter_b200/task_metrics.py derain_scores,
+ * sidd_scores, ycbcr_y), restated from the scripts and MATLAB's documented algorithms (unverified against MATLAB).
+ * Same descriptor table as the task metrics above: pred fp64 [H, W, 3], gt uint8 [H, W, 3].
+ *  pk_ycbcr_y          out uint8 [npix] = the Y channel of MATLAB rgb2ycbcr of rgb uint8 [npix, 3]: K1 R + K2 G + K3 B
+ *                      + 16 in fp64 with Ki = (1/255) * {65.481, 128.553, 24.966}, summed left to right without FMA,
+ *                      rounded half away from zero, saturated.
+ *  pk_derain_scores    psnr, ssim fp64 [n]: Painter/eval/derain/evaluate_PSNR_SSIM.m compute_psnr and SSIM_index on the
+ *                      Y channels of u = uint8(trunc(clip(pred, 0, 1) * 255)) and gt; C1 = (0.01 * 255)^2, C2 =
+ *                      (0.03 * 255)^2 as c1, c2; taps fp64 [11] the normalised 1-D Gaussian (sigma 1.5) whose outer
+ *                      product is the SSIM window.  Every image is at least 11 x 11.
+ *  pk_sidd_scores      psnr, ssim fp64 [n]: MATLAB psnr and ssim as Painter/eval/sidd/eval_sidd.m calls them, x =
+ *                      single(clip(pred, 0, 1)), y = single(gt) / 255 (H x W x 3 volume, replicate padding); consts fp64
+ *                      [20]: the 11 taps, then the 3 x 3 depth-filter matrix row by row; c1 = 0.01^2, c2 = 0.03^2.
+ *  Both: max_h, max_w bound every H, W; counters_zeroed uint32 [n] (zero on entry); partials fp64
+ *  [n * pk_{derain,sidd}_ws_doubles(max_h, max_w)].  One CTA per (16 x 16 tile, image); bitwise reproducible.    */
+int pk_ycbcr_y(const uint8_t* rgb, long long npix, uint8_t* out, void* stream);
+long long pk_derain_ws_doubles(int max_h, int max_w);
+long long pk_sidd_ws_doubles(int max_h, int max_w);
+int pk_derain_scores(const long long* items, const void* base, int n, int max_h, int max_w, const double* taps,
+                     unsigned* counters_zeroed, double* partials, double c1, double c2, double* psnr, double* ssim,
+                     void* stream);
+int pk_sidd_scores(const long long* items, const void* base, int n, int max_h, int max_w, const double* consts,
+                   unsigned* counters_zeroed, double* partials, double c1, double c2, double* psnr, double* ssim,
+                   void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * COCO panoptic post-processing (csrc/panoptic.cu, painter_b200/panoptic.py): Painter/eval/coco_panoptic's instance
  * decoding, matrix NMS, class vote and panoptic merge on the device.  A launch covers a batch of n images described by
  * an int64 device table, one row of PK_PANO_FIELDS per image: [pixels, staged, H, W].  pixels is the uint8 [H, W, 3]

@@ -7,6 +7,9 @@ painter_inference.run_batch without writing or reading PNG files (kernels in csr
                         mACC, pACC
     DepthMeter          Painter/eval/nyuv2_depth/eval_with_pngs.py as eval/nyuv2_depth/eval.sh runs it
     restoration_scores  the PSNR / SSIM of Painter/eval/lol/painter_inference_lol.py (skimage 0.19)
+    derain_scores       the PSNR / SSIM of Painter/eval/derain/evaluate_PSNR_SSIM.m (MATLAB; csrc/restoration_matlab.cu)
+    sidd_scores         the PSNR / SSIM of Painter/eval/sidd/eval_sidd.m (MATLAB psnr / ssim)
+    ycbcr_y             MATLAB rgb2ycbcr's Y channel of uint8 RGB, as derain_scores computes it
 
 Every update / call validates its host-side inputs on the host (ValueError) before any device work, then makes one
 upload (the host arrays and a descriptor table of every image's device address and size) and one launch for the whole
@@ -285,3 +288,97 @@ def restoration_scores(restored, gts, device="cuda"):
                                       ctypes.c_void_p(res[1].data_ptr()), _stream()), "pk_restoration_scores")
     host = res.cpu().numpy()
     return host[0].copy(), host[1].copy()
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# The two benchmarks the reference scores in MATLAB.  Restated from the scripts and MATLAB's documented algorithms,
+# unverified against MATLAB itself (DESIGN.md, Task metrics).
+_GAUSS_TAPS, _GAUSS_SIGMA = 11, 1.5
+_DERAIN_C1, _DERAIN_C2 = (0.01 * 255) ** 2, (0.03 * 255) ** 2
+_SIDD_C1, _SIDD_C2 = 0.01 ** 2, 0.03 ** 2
+
+
+def _gauss_taps():
+    """The normalised 1-D Gaussian of 11 taps, sigma 1.5: imgaussfilt's kernel, and the factor of fspecial('gaussian',
+    11, 1.5) (its outer product with itself; the values fspecial zeroes, below eps * max, do not occur here)."""
+    x = np.arange(_GAUSS_TAPS, dtype=np.float64) - _GAUSS_TAPS // 2
+    g = np.exp(-(x * x) / (2.0 * _GAUSS_SIGMA * _GAUSS_SIGMA))
+    return g / g.sum()
+
+
+def _depth_matrix(taps, depth=3):
+    """The depth pass of the separable Gaussian with replicate padding on `depth` planes, as a matrix: M[c, d] = the
+    sum of the taps whose clamped source plane is d."""
+    r = len(taps) // 2
+    M = np.zeros((depth, depth))
+    for c in range(depth):
+        for k, t in enumerate(taps):
+            M[c, min(max(c + k - r, 0), depth - 1)] += t
+    return M
+
+
+def ycbcr_y(img_u8):
+    """img_u8: device uint8 [H, W, 3] -> device uint8 [H, W]: the Y channel of MATLAB rgb2ycbcr, K1 R + K2 G + K3 B + 16
+    with Ki = (1/255) * (65.481, 128.553, 24.966)_i in fp64, summed left to right, rounded half away from zero."""
+    if not (torch.is_tensor(img_u8) and img_u8.is_cuda and img_u8.dtype == torch.uint8 and img_u8.dim() == 3
+            and img_u8.shape[2] == 3 and img_u8.is_contiguous() and img_u8.numel() > 0):
+        raise ValueError("ycbcr_y: img must be a contiguous device uint8 [H, W, 3] tensor")
+    out = torch.empty(img_u8.shape[:2], dtype=torch.uint8, device=img_u8.device)
+    check(lib().pk_ycbcr_y(ctypes.c_void_p(img_u8.data_ptr()), ctypes.c_longlong(out.numel()),
+                           ctypes.c_void_p(out.data_ptr()), _stream()), "pk_ycbcr_y")
+    return out
+
+
+def _matlab_scores(name, restored, gts, device, consts, c1, c2):
+    dev = _device(device)
+    n = len(restored)
+    counters = np.zeros(n, dtype=np.uint32)
+    upload, max_h, max_w = _batch(restored, gts, np.float64, np.uint8, 3, 3, dev, f"{name}_scores",
+                                  extra=(consts, counters))
+    views = upload()
+    ws_fn = getattr(lib(), f"pk_{name}_ws_doubles")
+    ws_fn.restype = ctypes.c_longlong
+    ws = int(ws_fn(max_h, max_w))
+    partials = torch.empty(n * ws, dtype=torch.float64, device=dev)
+    res = torch.empty((2, n), dtype=torch.float64, device=dev)
+    check(getattr(lib(), f"pk_{name}_scores")(
+        ctypes.c_void_p(views[0].data_ptr()), ctypes.c_void_p(views[0].data_ptr()), n, max_h, max_w,
+        ctypes.c_void_p(views[-2].data_ptr()), ctypes.c_void_p(views[-1].data_ptr()),
+        ctypes.c_void_p(partials.data_ptr()), ctypes.c_double(c1), ctypes.c_double(c2),
+        ctypes.c_void_p(res[0].data_ptr()), ctypes.c_void_p(res[1].data_ptr()), _stream()), f"pk_{name}_scores")
+    host = res.cpu().numpy()
+    return host[0].copy(), host[1].copy()
+
+
+def derain_scores(restored, gts, device="cuda"):
+    """Per-image PSNR and SSIM of Painter/eval/derain/evaluate_PSNR_SSIM.m on the PNGs painter_inference_derain.py
+    writes from run_one_image's output.
+
+    restored: float64 [H, W, 3] arrays (as run_batch(task="restore") returns them, or device tensors); gts: the uint8
+    [H, W, 3] decoded targets on the host; every image at least 11 x 11.  Returns (psnr, ssim), float64 numpy [n] each.
+
+    Prediction u = uint8(trunc(clip(x, 0, 1) * 255)) in fp64 (the script's PNG); both images go to the Y channel of
+    rgb2ycbcr (ycbcr_y).  PSNR = 20 log10(255 / sqrt(mean((Yp - Yg)^2))), the sum of squares exact in int64, +Inf for
+    identical images.  SSIM = SSIM_index's defaults: fspecial('gaussian', 11, 1.5) window, 'valid' filtering of Y, Y^2
+    and Yp Yg in fp64, C1 = (0.01 * 255)^2, C2 = (0.03 * 255)^2, the mean of the (H - 10) x (W - 10) map.  The script
+    averages per set and then over the five sets; that aggregation is the caller's (INTEGRATION.md)."""
+    for i, g in enumerate(gts):
+        if len(np.shape(g)) >= 2 and min(np.shape(g)[:2]) < _GAUSS_TAPS:
+            raise ValueError(f"derain_scores: image {i} is {np.shape(g)[:2]}; SSIM_index needs at least 11 x 11")
+    return _matlab_scores("derain", restored, gts, device, _gauss_taps(), _DERAIN_C1, _DERAIN_C2)
+
+
+def sidd_scores(restored, gts, device="cuda"):
+    """Per-block PSNR and SSIM of Painter/eval/sidd/eval_sidd.m on the Idenoised.mat painter_inference_sidd.py saves.
+
+    restored: float64 [H, W, 3] arrays (as run_batch(task="restore") returns them, or device tensors); gts: uint8
+    [H, W, 3] host arrays.  Returns (psnr, ssim), float64 numpy [n] each; eval_sidd.m reports their means.
+
+    x = single(clip(r, 0, 1)) (the .mat holds float32), y = im2single(g) = single(g) / 255.  PSNR =
+    10 log10(1 / mean((x - y)^2)) over the 3 H W values (peak 1), in fp64.  SSIM = MATLAB ssim on the H x W x 3 array,
+    which it filters as a volume: a separable Gaussian (sigma 1.5, 11 taps) with replicate padding along rows, columns
+    and depth ('same' output), C1 = 0.01^2, C2 = 0.03^2, the mean of the map; the depth pass on 3 planes is a 3 x 3
+    matrix applied after the 2-D passes.  MATLAB computes in single precision, this in fp64."""
+    taps = _gauss_taps()
+    consts = np.concatenate([taps, _depth_matrix(taps).reshape(-1)])
+    return _matlab_scores("sidd", restored, gts, device, consts, _SIDD_C1, _SIDD_C2)

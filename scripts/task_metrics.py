@@ -10,14 +10,24 @@ weights) for both arms.
            eval_with_pngs.eval() (eval.sh's arguments)
            ours:      run_batch(task="depth") -> DepthMeter.update on the device maps
            NYUv2-sized images (640 x 480)
+    derain reference: run_batch(task="restore"), the PNG painter_inference_derain.py writes ((clip(x, 0, 1) * 255)
+           .astype(uint8)) written and read back with PIL, then oracle/matlab_ref.py's restatement of
+           evaluate_PSNR_SSIM.m on the CPU (standing in for MATLAB)
+           ours:      run_batch(task="restore") -> derain_scores
+           Rain100-sized images (481 x 321 and 321 x 481)
+    sidd   reference: run_batch(task="restore"), the float32 array painter_inference_sidd.py saves, then
+           oracle/matlab_ref.py's restatement of eval_sidd.m's psnr / ssim on the CPU
+           ours:      run_batch(task="restore") -> sidd_scores
+           SIDD blocks (256 x 256)
 
 For each task and arm it processes --images images (after one warm-up batch that captures the CUDA graph) and prints
 one JSON line: images/s end to end (host clock; the metric state is on the host or synchronised at the end) and the
 metric step alone in ms per image (CUDA events around the metric calls, the inference outputs already computed).  The
-two semseg arms' confusion matrices are asserted equal, and the two depth arms' d1, d2, d3 (float32) likewise.  The
+two semseg arms' confusion matrices are asserted equal, and the two depth arms' d1, d2, d3 (float32) likewise; the
+derain and sidd arms' PSNR to 1e-13 relative and SSIM to 1e-12.  The
 card's name, power limit and max SM clock come first.  Needs the staged reference (scripts/stage_reference.py).
 
-    python scripts/task_metrics.py [--images 64] [--batch 8] [--out task_metrics.jsonl]
+    python scripts/task_metrics.py [--images 64] [--batch 8] [--tasks segm,depth,derain,sidd] [--out task_metrics.jsonl]
 """
 import argparse
 import json
@@ -42,6 +52,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--images", type=int, default=64, help="images per timed window and arm")
     ap.add_argument("--batch", type=int, default=8, help="images per run_batch call")
+    ap.add_argument("--tasks", default="segm,depth,derain,sidd")
     ap.add_argument("--out", default="")
     args = ap.parse_args()
     import cv2
@@ -52,11 +63,13 @@ def main():
     from _common import build_model
     from oracle import painter_oracle as po
     from painter_b200 import painter_inference as pi
-    from painter_b200.task_metrics import DepthMeter, SemSegMeter
+    from oracle import matlab_ref as mr
+    from painter_b200.task_metrics import DepthMeter, SemSegMeter, derain_scores, sidd_scores
 
     if not torch.cuda.is_available():
         raise SystemExit("task_metrics: needs a GPU")
     print("card (name, power limit, max SM clock):", card(), flush=True)
+    tasks = set(args.tasks.split(","))
     n_img, B = args.images, args.batch
     n_calls = (n_img + B - 1) // B
     dev = torch.device("cuda")
@@ -173,22 +186,73 @@ def main():
         emit({"task": task, "arm": name, "images": n_calls * B, "batch": B, "img_s": round(n_calls * B / wall, 2),
               "metric_ms_per_img": round(ev.ms() / (n_calls * B), 3)})
 
-    arm("segm", "reference (PNG, PIL, post_process_segm_output, bincount)", seg_ref_acc)
-    sm = SemSegMeter(palette)
-    arm("segm", "run_batch -> SemSegMeter", seg_ours(sm))
-    # both arms' state holds the warm-up batch and the timed ones: the same 1 + n_calls batches
-    np.testing.assert_array_equal(sm.conf_matrix, ref_conf)
-    emit({"task": "segm", "confusion_matrices_equal": True, "pixels": int(ref_conf.sum())})
+    if "segm" in tasks:
+        arm("segm", "reference (PNG, PIL, post_process_segm_output, bincount)", seg_ref_acc)
+        sm = SemSegMeter(palette)
+        arm("segm", "run_batch -> SemSegMeter", seg_ours(sm))
+        # both arms' state holds the warm-up batch and the timed ones: the same 1 + n_calls batches
+        np.testing.assert_array_equal(sm.conf_matrix, ref_conf)
+        emit({"task": "segm", "confusion_matrices_equal": True, "pixels": int(ref_conf.sum())})
 
-    arm("depth", "reference (PNG, cv2, eval_with_pngs.eval)", dep_reference)
-    dm = DepthMeter()
-    arm("depth", "run_batch -> DepthMeter", dep_ours(dm))
-    # columns of eval(): silog, log10, abs_rel, sq_rel, rms, log_rms, d1, d2, d3
-    ref = np.concatenate(ref_depth)
-    ours = dm.per_image()
-    np.testing.assert_array_equal(ours[:, :3].astype(np.float32), ref[:, 6:9])
-    np.testing.assert_allclose(ours[:, 3:], ref[:, [2, 3, 4, 5, 0, 1]], rtol=1e-5)
-    emit({"task": "depth", "d1_d2_d3_equal": True, "others_within_1e-5": True, "images": len(ours)})
+    if "depth" in tasks:
+        arm("depth", "reference (PNG, cv2, eval_with_pngs.eval)", dep_reference)
+        dm = DepthMeter()
+        arm("depth", "run_batch -> DepthMeter", dep_ours(dm))
+        # columns of eval(): silog, log10, abs_rel, sq_rel, rms, log_rms, d1, d2, d3
+        ref = np.concatenate(ref_depth)
+        ours = dm.per_image()
+        np.testing.assert_array_equal(ours[:, :3].astype(np.float32), ref[:, 6:9])
+        np.testing.assert_allclose(ours[:, 3:], ref[:, [2, 3, 4, 5, 0, 1]], rtol=1e-5)
+        emit({"task": "depth", "d1_d2_d3_equal": True, "others_within_1e-5": True, "images": len(ours)})
+
+    # ---------------- derain and SIDD (scored in MATLAB by the reference) ----------------
+    def restoration(task, sizes, ref_score, ours_score):
+        rgts = []
+        for j in range(B):
+            w, h = sizes[j % len(sizes)]
+            rgts.append(rng.randint(0, 256, size=(h, w, 3)).astype(np.uint8))
+        ref_out, ours_out = [], []
+
+        def reference(k, ev):
+            with torch.no_grad():
+                outs = run("restore", sizes, k)
+            with ev:
+                ref_out.extend(ref_score(k, j, o, g) for j, (o, g) in enumerate(zip(outs, rgts)))
+
+        def ours(k, ev):
+            with torch.no_grad():
+                outs = run("restore", sizes, k)
+            with ev:
+                ours_out.append(np.stack(ours_score(outs, rgts), 1))
+
+        return reference, ours, ref_out, ours_out
+
+    def derain_ref(k, j, o, g):
+        path = os.path.join(tmp, f"r{k}_{j}.png")
+        Image.fromarray((np.clip(o, 0, 1) * 255).astype(np.uint8)).save(path)
+        return mr.derain_scores_u8(np.array(Image.open(path)), g)
+
+    def sidd_ref(k, j, o, g):
+        x, y = mr.sidd_inputs(o, g)
+        return mr.sidd_psnr(x, y), mr.sidd_ssim(x, y)
+
+    for task, sizes, ref_score, ours_score, ref_name in [
+            ("derain", [(481, 321), (321, 481)], derain_ref, derain_scores,
+             "reference (PNG, PIL, evaluate_PSNR_SSIM.m restated on the CPU)"),
+            ("sidd", [(256, 256)], sidd_ref, sidd_scores, "reference (float32 array, eval_sidd.m restated on the CPU)")]:
+        if task not in tasks:
+            continue
+        reference, ours, ref_out, ours_out = restoration(task, sizes, ref_score, ours_score)
+        arm(task, ref_name, reference)
+        arm(task, f"run_batch -> {ours_score.__name__}", ours)
+        ref, mine = np.array(ref_out), np.concatenate(ours_out)
+        assert ref.shape == mine.shape, (ref.shape, mine.shape)
+        fin = np.isfinite(ref[:, 0])
+        assert np.array_equal(np.isfinite(mine[:, 0]), fin)
+        assert np.all(np.abs(mine[fin, 0] - ref[fin, 0]) <= 1e-13 * np.abs(ref[fin, 0])), "PSNR"
+        assert np.all(np.abs(mine[:, 1] - ref[:, 1]) <= 1e-12), "SSIM"
+        emit({"task": task, "psnr_within_1e-13_rel": True, "ssim_within_1e-12": True, "images": len(ref),
+              "mean_psnr": float(np.mean(mine[:, 0])), "mean_ssim": float(np.mean(mine[:, 1]))})
 
 
 if __name__ == "__main__":
