@@ -267,46 +267,35 @@ int pk_set_pdl(int on);
  *                       (:75-91 stitch + ImageNet normalisation, :29-34 nhwc->nchw .float()); host arrays of P device
  *                       pointers
  *  pk_nhwc_to_nchw_f32  torch.einsum('nhwc->nchw', x).float() of an already normalised fp64/fp32 batch (:29-34)
- *  pk_seg_postprocess   out fp64 [h*p/2, w*p, 3] = clip((unpatchify(patch)[0, bottom half] * std + mean) * 255, 0, 255)
- *                       (:48-52); bin (nullable) fp32 [h*p/2, w*p] = mean_c(out) > 128 (:164-169, video cache)
- *  pk_nearest_blend     dst uint8 [OH,OW,3] = uint8(image * (0.6 * nearest(seg) / 255 + 0.4)) (:93-102)
- *  pk_bilinear_u8       dst uint8 [OH,OW,3] = uint8(int(bilinear(seg))) (painter_inference_segm.py:89-92)
- *  pk_denorm_bottom     out fp64 [h*p/2, w*p, 3] = finish(unpatchify(patch)[0, bottom half] * std + mean); finish:
- *                       0 = clip(x * 255, 0, 255) (pk_seg_postprocess without bin), 1 = clip(x * 10000, 0, 10000)
- *                       (painter_inference_depth.py), 2 = x (painter_inference_{sidd,lol,derain}.py)
- *  pk_bicubic_f64       dst fp64 [OH,OW,3] = F.interpolate(src, mode='bicubic') as torch-CPU computes it on the
- *                       float64 channels-last tensor, unclipped ({sidd,lol,derain} run_one_image, the returned array)
- *  pk_depth_finish      dst int32 [OH,OW] = int(bilinear(src).mean(-1)) (painter_inference_depth.py run_one_image);
- *                       cl_form selects torch-CPU's channels-last summation order (it takes that kernel on one
- *                       thread or when OH + OW <= 128), else its generic one
- *  pk_nearest_u8        dst uint8 [OH,OW,3] = uint8(int(nearest(src))) (painter_inference_pano_inst.py,
- *                       painter_inference_pose.py run_one_image); cl_form selects torch-CPU's channels-last source
- *                       index (it takes that kernel when OH + OW <= 128), else its generic one
  * pk_stitch_normalize takes any number of members (launched in chunks of 16).
- * Batched inference (many canvases per forward, painter_inference.run_batch, seggpt_engine.segment_batch):
- *  pk_denorm_bottom_batched  out fp64 [B, h*p/2, w*p, 3]: pk_denorm_bottom of samples 0, src_stride, 2 src_stride, ..
- *                       of patch; bin (nullable, finish 0 only) fp32 [B, h*p/2, w*p] as in pk_seg_postprocess
- *  pk_finish_ragged     one launch finishing n images of different output sizes from src fp64 [*, SH, SW, 3] with the
- *                       per-pixel code of the single-image kernel of `op` (PK_FIN_*).  items: int32 device table, one
- *                       row of PK_RAG_FIELDS per image: [src sample, OH, OW, cl_form, offset lo, hi]; the image's
- *                       output starts at dst + offset (elements of the op's output type: uint8, int32 for the depth,
- *                       fp64 for the bicubic) and, for the blend, its source image uint8 [OH, OW, 3] at image + offset
- *                       (image is null for every other op).  cl_form as in the single-image call (nearest_u8, depth).
- *                       max_pix >= every OH * OW sizes the grid.                                                    */
+ * De-normalisation and finishing, one launch for a whole batch (the per-image wrappers pass one image):
+ *  pk_denorm_bottom_batched  out fp64 [B, h*p/2, w*p, 3] = finish(unpatchify(patch)[b * src_stride, bottom half]
+ *                       * std + mean) (:48-52); finish: 0 = clip(x * 255, 0, 255), 1 = clip(x * 10000, 0, 10000)
+ *                       (painter_inference_depth.py), 2 = x (painter_inference_{sidd,lol,derain}.py); bin (nullable,
+ *                       finish 0 only) fp32 [B, h*p/2, w*p] = mean_c(out) > 128 (:164-169, video cache)
+ *  pk_finish_ragged     one launch finishing n images of different output sizes from src fp64 [*, SH, SW, 3] with
+ *                       `op` (PK_FIN_*).  items: int32 device table, one row of PK_RAG_FIELDS per image: [src sample,
+ *                       OH, OW, cl_form, offset lo, hi]; the image's output starts at dst + offset (elements of the
+ *                       op's output type: uint8, int32 for the depth, fp64 for the bicubic) and, for the blend, its
+ *                       source image uint8 [OH, OW, 3] at image + offset (image is null for every other op).
+ *                       max_pix >= every OH * OW sizes the grid.  The ops, as torch-CPU computes them on the float64
+ *                       channels-last tensor:
+ *     PK_FIN_BILINEAR_U8    dst uint8 [OH,OW,3] = uint8(int(bilinear(src))) (painter_inference_segm.py:89-92)
+ *     PK_FIN_NEAREST_U8     dst uint8 [OH,OW,3] = uint8(int(nearest(src))) (painter_inference_pano_inst.py,
+ *                           painter_inference_pose.py); cl_form selects torch-CPU's channels-last source index (it
+ *                           takes that kernel when OH + OW <= 128), else its generic one
+ *     PK_FIN_DEPTH          dst int32 [OH,OW] = int(bilinear(src).mean(-1)) (painter_inference_depth.py); cl_form
+ *                           selects torch-CPU's channels-last summation order (it takes that kernel on one thread or
+ *                           when OH + OW <= 128), else its generic one
+ *     PK_FIN_BICUBIC_F64    dst fp64 [OH,OW,3] = F.interpolate(src, mode='bicubic'), unclipped
+ *                           ({sidd,lol,derain} run_one_image, the returned array)
+ *     PK_FIN_NEAREST_BLEND  dst uint8 [OH,OW,3] = uint8(image * (0.6 * nearest(src) / 255 + 0.4)) (:93-102)     */
 enum { PK_RAG_FIELDS = 6 };
 enum { PK_FIN_BILINEAR_U8 = 0, PK_FIN_NEAREST_U8 = 1, PK_FIN_DEPTH = 2, PK_FIN_BICUBIC_F64 = 3,
        PK_FIN_NEAREST_BLEND = 4 };
 int pk_stitch_normalize(const void* const* top, const int* top_dtype, const void* const* bottom,
                         const int* bottom_dtype, float* out, int P, int S, void* stream);
 int pk_nhwc_to_nchw_f32(const void* in, int in_is_f64, float* out, int n, int H, int W, void* stream);
-int pk_seg_postprocess(const float* patch, double* out, float* bin_or_null, int h, int w, int p, void* stream);
-int pk_nearest_blend(const double* seg, int SH, int SW, const uint8_t* image, uint8_t* dst, int OH, int OW,
-                     void* stream);
-int pk_bilinear_u8(const double* seg, int SH, int SW, uint8_t* dst, int OH, int OW, void* stream);
-int pk_denorm_bottom(const float* patch, double* out, int h, int w, int p, int finish, void* stream);
-int pk_bicubic_f64(const double* src, int SH, int SW, double* dst, int OH, int OW, void* stream);
-int pk_depth_finish(const double* src, int SH, int SW, int32_t* dst, int OH, int OW, int cl_form, void* stream);
-int pk_nearest_u8(const double* src, int SH, int SW, uint8_t* dst, int OH, int OW, int cl_form, void* stream);
 int pk_denorm_bottom_batched(const float* patch, double* out, float* bin_or_null, int B, int src_stride, int h, int w,
                              int p, int finish, void* stream);
 int pk_finish_ragged(int op, const double* src, int SH, int SW, const int* items, int n, int max_pix,

@@ -81,7 +81,7 @@ enum DenormFinish { kClip255 = 0, kClip10000 = 1, kPlain = 2 };
 // patch: patchified prediction [*, h*w, p*p*3] fp32 (inner order (pr, pc, c), models_painter.py:355-368);
 // = unpatchify -> 'nchw->nhwc' -> bottom half -> de-normalise (seggpt_engine.py:48-52).  Optionally (kClip255 only)
 // also writes bin[b, y, x] = (mean_c(out) > 128) (the video path's next-frame target, seggpt_engine.py:164-169).
-// The single-image entry points run it with B = 1; every sample's pixels get the same arithmetic.
+// Every sample gets the same arithmetic whatever B and src_stride are, so sample b equals a B = 1 call on it alone.
 template <int kFinish>
 __global__ void __launch_bounds__(256)
 seg_postprocess_kernel(const float* __restrict__ patch, double* __restrict__ out, float* __restrict__ bin, int B,
@@ -125,8 +125,8 @@ __device__ __forceinline__ int nearest_idx(int dst, int in_size, int out_size) {
 }
 // dst[y, x, c] (uint8 [OH, OW, 3]) = uint8(image[y, x, c] * (0.6 * nearest(seg)[y, x, c] / 255 + 0.4))
 // (seggpt_engine.py:97-102: F.interpolate(mode='nearest') to the original size, alpha blend, astype(uint8)).
-// The *_at functions compute output element i of one image; the single-image kernel and the ragged kernel
-// (ragged_finish_kernel) both call them, so a batched result is the single-image result.
+// The *_at functions compute output element i of one image; ragged_finish_kernel calls them with each image's own
+// source sample, size and output.
 __device__ __forceinline__ void nearest_blend_at(const double* __restrict__ seg, int SH, int SW,
                                                  const uint8_t* __restrict__ image, uint8_t* __restrict__ dst, int OH,
                                                  int OW, size_t i) {
@@ -137,14 +137,6 @@ __device__ __forceinline__ void nearest_blend_at(const double* __restrict__ seg,
   const double o = seg[(static_cast<size_t>(sy) * SW + sx) * 3 + c];
   const double v = __dmul_rn(static_cast<double>(image[i]), __dadd_rn(__dmul_rn(0.6, o) / 255.0, 0.4));
   dst[i] = static_cast<uint8_t>(v);   // numpy astype(uint8): truncation (values are within [0, 255])
-}
-__global__ void __launch_bounds__(256)
-nearest_blend_kernel(const double* __restrict__ seg, int SH, int SW, const uint8_t* __restrict__ image,
-                     uint8_t* __restrict__ dst, int OH, int OW) {
-  const size_t total = static_cast<size_t>(OH) * OW * 3;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x)
-    nearest_blend_at(seg, SH, SW, image, dst, OH, OW, i);
 }
 
 // One axis of ATen's linear interpolation (align_corners=False, scale = in / out from the sizes):
@@ -187,13 +179,6 @@ __device__ __forceinline__ void bilinear_u8_at(const double* __restrict__ seg, i
                    ty.l1 * (tx.l0 * at(ty.i1, tx.i0) + tx.l1 * at(ty.i1, tx.i1));
   dst[i] = static_cast<uint8_t>(static_cast<int>(v));
 }
-__global__ void __launch_bounds__(256)
-bilinear_u8_kernel(const double* __restrict__ seg, int SH, int SW, uint8_t* __restrict__ dst, int OH, int OW) {
-  const size_t total = static_cast<size_t>(OH) * OW * 3;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x)
-    bilinear_u8_at(seg, SH, SW, dst, OH, OW, i);
-}
 
 // dst[y, x] (int32 [OH, OW]) = int(mean_c(bilinear(src)[y, x, c]))   (nyuv2_depth/painter_inference_depth.py:
 // F.interpolate(mode='bilinear') on the float64 tensor, .mean(-1), .int()).  torch-CPU evaluates the 2 x 2 sum in one
@@ -227,14 +212,6 @@ __device__ __forceinline__ void depth_finish_at(const double* __restrict__ src, 
   }
   dst[i] = static_cast<int32_t>(__ddiv_rn(s, 3.0));   // .int(): truncation (values are within [0, 10000])
 }
-__global__ void __launch_bounds__(256)
-depth_finish_kernel(const double* __restrict__ src, int SH, int SW, int32_t* __restrict__ dst, int OH, int OW,
-                    int cl_form) {
-  const size_t total = static_cast<size_t>(OH) * OW;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x)
-    depth_finish_at(src, SH, SW, dst, OH, OW, cl_form, i);
-}
 
 // ATen's nearest source index in its generic kernel (HelperInterpNearest): scale = double(in) / out, then
 // floorf(scale * dst) of the product rounded to float.  Its channels-last kernel uses nearest_idx above instead.
@@ -256,14 +233,6 @@ __device__ __forceinline__ void nearest_u8_at(const double* __restrict__ src, in
   const int sy = cl_form ? nearest_idx(y, SH, OH) : nearest_idx_generic(y, SH, sch);
   const int sx = cl_form ? nearest_idx(x, SW, OW) : nearest_idx_generic(x, SW, scw);
   dst[i] = static_cast<uint8_t>(static_cast<int>(src[(static_cast<size_t>(sy) * SW + sx) * 3 + c]));
-}
-__global__ void __launch_bounds__(256)
-nearest_u8_kernel(const double* __restrict__ src, int SH, int SW, uint8_t* __restrict__ dst, int OH, int OW,
-                  int cl_form) {
-  const size_t total = static_cast<size_t>(OH) * OW * 3;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x)
-    nearest_u8_at(src, SH, SW, dst, OH, OW, cl_form, i);
 }
 
 // ATen's cubic convolution weights (get_cubic_upsample_coefficients, A = -0.75) of the 4 taps around a source
@@ -330,13 +299,6 @@ __device__ __forceinline__ void bicubic_f64_at(const double* __restrict__ src, i
   }
   dst[i] = cubic_sum(rows, ky.w);
 }
-__global__ void __launch_bounds__(256)
-bicubic_f64_kernel(const double* __restrict__ src, int SH, int SW, double* __restrict__ dst, int OH, int OW) {
-  const size_t total = static_cast<size_t>(OH) * OW * 3;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x)
-    bicubic_f64_at(src, SH, SW, dst, OH, OW, i);
-}
 
 // Ragged finish of a batch: one CTA row (blockIdx.y) per descriptor row [src sample, OH, OW, cl_form, offset lo, hi]
 // (PK_RAG_FIELDS), grid-stride over that image's output elements.  src sample s is src + s * SH * SW * 3; the image's
@@ -371,20 +333,6 @@ static inline int stream_grid(size_t total) {
   size_t g = (total + 255) / 256;
   const size_t cap = static_cast<size_t>(sm_count()) * 16;
   return static_cast<int>(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
-static int denorm_launch(const float* patch, double* out, float* bin, int B, int src_stride, int h, int w, int p,
-                         int finish, void* stream, const char* name) {
-  const size_t total = static_cast<size_t>(B) * h * p / 2 * w * p;
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (finish == kClip255)
-    seg_postprocess_kernel<kClip255><<<stream_grid(total), 256, 0, st>>>(patch, out, bin, B, src_stride, h, w, p);
-  else if (finish == kClip10000)
-    seg_postprocess_kernel<kClip10000><<<stream_grid(total), 256, 0, st>>>(patch, out, bin, B, src_stride, h, w, p);
-  else
-    seg_postprocess_kernel<kPlain><<<stream_grid(total), 256, 0, st>>>(patch, out, bin, B, src_stride, h, w, p);
-  PK_LAUNCH_CHECK(name);
-  return 0;
 }
 
 }  // namespace pk
@@ -424,70 +372,20 @@ extern "C" int pk_nhwc_to_nchw_f32(const void* in, int in_is_f64, float* out, in
   return 0;
 }
 
-extern "C" int pk_seg_postprocess(const float* patch, double* out, float* bin_or_null, int h, int w, int p,
-                                  void* stream) {
-  PK_CHECK(patch && out && h > 0 && w > 0 && p > 0 && h % 2 == 0, "pk_seg_postprocess: bad arguments");
-  const size_t total = static_cast<size_t>(h) * p / 2 * w * p;
-  seg_postprocess_kernel<kClip255><<<stream_grid(total), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      patch, out, bin_or_null, 1, 1, h, w, p);
-  PK_LAUNCH_CHECK("pk_seg_postprocess");
-  return 0;
-}
-
-extern "C" int pk_denorm_bottom(const float* patch, double* out, int h, int w, int p, int finish, void* stream) {
-  PK_CHECK(patch && out && h > 0 && w > 0 && p > 0 && h % 2 == 0 && finish >= kClip255 && finish <= kPlain,
-           "pk_denorm_bottom: bad arguments");
-  return denorm_launch(patch, out, nullptr, 1, 1, h, w, p, finish, stream, "pk_denorm_bottom");
-}
-
 extern "C" int pk_denorm_bottom_batched(const float* patch, double* out, float* bin_or_null, int B, int src_stride,
                                         int h, int w, int p, int finish, void* stream) {
   PK_CHECK(patch && out && B >= 1 && src_stride >= 1 && h > 0 && w > 0 && p > 0 && h % 2 == 0 && finish >= kClip255 &&
                finish <= kPlain, "pk_denorm_bottom_batched: bad arguments");
   PK_CHECK(!bin_or_null || finish == kClip255, "pk_denorm_bottom_batched: the binarised mask needs finish 0 (x 255)");
-  return denorm_launch(patch, out, bin_or_null, B, src_stride, h, w, p, finish, stream, "pk_denorm_bottom_batched");
-}
-
-extern "C" int pk_nearest_blend(const double* seg, int SH, int SW, const uint8_t* image, uint8_t* dst, int OH, int OW,
-                                void* stream) {
-  PK_CHECK(seg && image && dst && SH > 0 && SW > 0 && OH > 0 && OW > 0, "pk_nearest_blend: bad arguments");
-  nearest_blend_kernel<<<stream_grid(static_cast<size_t>(OH) * OW * 3), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      seg, SH, SW, image, dst, OH, OW);
-  PK_LAUNCH_CHECK("pk_nearest_blend");
-  return 0;
-}
-
-extern "C" int pk_bilinear_u8(const double* seg, int SH, int SW, uint8_t* dst, int OH, int OW, void* stream) {
-  PK_CHECK(seg && dst && SH > 0 && SW > 0 && OH > 0 && OW > 0, "pk_bilinear_u8: bad arguments");
-  bilinear_u8_kernel<<<stream_grid(static_cast<size_t>(OH) * OW * 3), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      seg, SH, SW, dst, OH, OW);
-  PK_LAUNCH_CHECK("pk_bilinear_u8");
-  return 0;
-}
-
-extern "C" int pk_bicubic_f64(const double* src, int SH, int SW, double* dst, int OH, int OW, void* stream) {
-  PK_CHECK(src && dst && SH > 0 && SW > 0 && OH > 0 && OW > 0, "pk_bicubic_f64: bad arguments");
-  bicubic_f64_kernel<<<stream_grid(static_cast<size_t>(OH) * OW * 3), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      src, SH, SW, dst, OH, OW);
-  PK_LAUNCH_CHECK("pk_bicubic_f64");
-  return 0;
-}
-
-extern "C" int pk_depth_finish(const double* src, int SH, int SW, int32_t* dst, int OH, int OW, int cl_form,
-                               void* stream) {
-  PK_CHECK(src && dst && SH > 0 && SW > 0 && OH > 0 && OW > 0, "pk_depth_finish: bad arguments");
-  depth_finish_kernel<<<stream_grid(static_cast<size_t>(OH) * OW), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      src, SH, SW, dst, OH, OW, cl_form != 0);
-  PK_LAUNCH_CHECK("pk_depth_finish");
-  return 0;
-}
-
-extern "C" int pk_nearest_u8(const double* src, int SH, int SW, uint8_t* dst, int OH, int OW, int cl_form,
-                             void* stream) {
-  PK_CHECK(src && dst && SH > 0 && SW > 0 && OH > 0 && OW > 0, "pk_nearest_u8: bad arguments");
-  nearest_u8_kernel<<<stream_grid(static_cast<size_t>(OH) * OW * 3), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      src, SH, SW, dst, OH, OW, cl_form != 0);
-  PK_LAUNCH_CHECK("pk_nearest_u8");
+  const int grid = stream_grid(static_cast<size_t>(B) * h * p / 2 * w * p);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (finish == kClip255)
+    seg_postprocess_kernel<kClip255><<<grid, 256, 0, st>>>(patch, out, bin_or_null, B, src_stride, h, w, p);
+  else if (finish == kClip10000)
+    seg_postprocess_kernel<kClip10000><<<grid, 256, 0, st>>>(patch, out, bin_or_null, B, src_stride, h, w, p);
+  else
+    seg_postprocess_kernel<kPlain><<<grid, 256, 0, st>>>(patch, out, bin_or_null, B, src_stride, h, w, p);
+  PK_LAUNCH_CHECK("pk_denorm_bottom_batched");
   return 0;
 }
 

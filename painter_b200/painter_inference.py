@@ -15,6 +15,9 @@ the host.
 The eval scripts call the model without torch.no_grad(), so a module in precision "auto" runs its bf16 training
 arithmetic there; these mirrors run under no_grad, which selects the fp32-accurate forward (and keeps no autograd
 state), as the ADE20k mirror always has.
+
+Each mirror is run_batch of its one image at forward batch 1: what run_batch returns or writes for an image is what
+the mirror returns or writes for it alone.  Canvases other than float32 / float64 are refused with a ValueError.
 """
 import ctypes
 
@@ -23,115 +26,31 @@ import torch
 
 from . import seggpt_engine as _se
 from ._lib import check, lib
-from .seggpt_engine import _graphed, _stream, seg_postprocess
+from .seggpt_engine import _graphed, _stream
 
-# pk_denorm_bottom finish codes
+# pk_denorm_bottom_batched finish codes
 CLIP255, CLIP10000, PLAIN = 0, 1, 2
-
-
-def bilinear_u8(seg, OH, OW):
-    """seg fp64 [SH, SW, 3] -> uint8 [OH, OW, 3] = uint8(int(F.interpolate(seg, mode='bilinear')))."""
-    dst = torch.empty((OH, OW, 3), dtype=torch.uint8, device=seg.device)
-    check(lib().pk_bilinear_u8(ctypes.c_void_p(seg.data_ptr()), seg.shape[0], seg.shape[1],
-                               ctypes.c_void_p(dst.data_ptr()), OH, OW, _stream()), "pk_bilinear_u8")
-    return dst
-
-
-def denorm_bottom(patch, h, w, p, finish):
-    """patchified prediction [B, h*w, p*p*3] fp32 -> fp64 [h*p/2, w*p, 3]: bottom half of sample 0, de-normalised,
-    then ×255 clipped (CLIP255), ×10000 clipped (CLIP10000) or left as is (PLAIN)."""
-    assert patch.dtype == torch.float32 and patch.is_contiguous()
-    out = torch.empty((h * p // 2, w * p, 3), dtype=torch.float64, device=patch.device)
-    check(lib().pk_denorm_bottom(ctypes.c_void_p(patch.data_ptr()), ctypes.c_void_p(out.data_ptr()), h, w, p, finish,
-                                 _stream()), "pk_denorm_bottom")
-    return out
-
-
-def nearest_u8(src, OH, OW):
-    """src fp64 [SH, SW, 3] -> uint8 [OH, OW, 3] = uint8(int(F.interpolate(src, mode='nearest'))).  torch-CPU
-    computes the source index in float from a float scale in its channels-last kernel (3 channels: OH + OW <= 128) and
-    from a double scale in its generic one; the same index is used here."""
-    dst = torch.empty((OH, OW, 3), dtype=torch.uint8, device=src.device)
-    cl_form = int(OH + OW <= 128)
-    check(lib().pk_nearest_u8(ctypes.c_void_p(src.data_ptr()), src.shape[0], src.shape[1],
-                              ctypes.c_void_p(dst.data_ptr()), OH, OW, cl_form, _stream()), "pk_nearest_u8")
-    return dst
-
-
-def depth_finish(src, OH, OW):
-    """src fp64 [SH, SW, 3] -> int32 [OH, OW] = F.interpolate(src, mode='bilinear').mean(-1).int().  torch-CPU sums
-    the 2 x 2 taps in its channels-last kernel's order on one thread or for OH + OW <= 128 (3 channels), else in its
-    generic kernel's order; the same order is used here, so the result is identical in either case."""
-    dst = torch.empty((OH, OW), dtype=torch.int32, device=src.device)
-    cl_form = int(torch.get_num_threads() == 1 or OH + OW <= 128)
-    check(lib().pk_depth_finish(ctypes.c_void_p(src.data_ptr()), src.shape[0], src.shape[1],
-                                ctypes.c_void_p(dst.data_ptr()), OH, OW, cl_form, _stream()), "pk_depth_finish")
-    return dst
-
-
-def bicubic_f64(src, OH, OW):
-    """src fp64 [SH, SW, 3] -> fp64 [OH, OW, 3] = F.interpolate(src, mode='bicubic') (align_corners=False, no clip)."""
-    dst = torch.empty((OH, OW, 3), dtype=torch.float64, device=src.device)
-    check(lib().pk_bicubic_f64(ctypes.c_void_p(src.data_ptr()), src.shape[0], src.shape[1],
-                               ctypes.c_void_p(dst.data_ptr()), OH, OW, _stream()), "pk_bicubic_f64")
-    return dst
-
-
-def _predict(img, tgt, model, device):
-    """The front half every eval script shares: img, tgt numpy [2*S, S, 3] ImageNet-normalised canvases ->
-    nchw fp32 on the device, the bottom-half mask, valid = 1, and one graphed forward of the module (or of the
-    `.module` of a DistributedDataParallel-style wrapper).  Returns (patchified prediction, h, w, p)."""
-    device = torch.device(device)
-    net = model.module if hasattr(model, "module") else model
-    x = torch.as_tensor(img).unsqueeze(0).to(device, non_blocking=True)
-    t = torch.as_tensor(tgt).unsqueeze(0).to(device, non_blocking=True)
-    _, H, W, _ = x.shape
-    xin = torch.empty((1, 3, H, W), dtype=torch.float32, device=device)
-    tin = torch.empty((1, 3, H, W), dtype=torch.float32, device=device)
-    for src, dst in ((x, xin), (t, tin)):
-        check(lib().pk_nhwc_to_nchw_f32(ctypes.c_void_p(src.data_ptr()), int(src.dtype == torch.float64),
-                                        ctypes.c_void_p(dst.data_ptr()), 1, H, W, _stream()), "pk_nhwc_to_nchw_f32")
-    p = net.patch_size
-    n = (H // p) * (W // p)
-    mask = torch.zeros(1, n, device=device)
-    mask[:, n // 2:] = 1
-    valid = torch.ones_like(tin)
-    _, y, _ = _graphed(net)(xin, tin, mask, valid)
-    return y, H // p, W // p, p
 
 
 @torch.no_grad()
 def run_one_image(img, tgt, size, model, out_path, device):
     """ADE20k semantic / COCO panoptic semseg.  img, tgt: numpy [2*S, S, 3] ImageNet-normalised canvases; size =
     (width, height) of the source image; model: the painter_b200 Painter module or a DistributedDataParallel wrapper
-    of it (the script passes `model.module` users).  Writes the uint8 PNG to out_path."""
-    from PIL import Image
-    y, h, w, p = _predict(img, tgt, model, device)
-    seg, _ = seg_postprocess(y, h, w, p)
-    out = bilinear_u8(seg, size[1], size[0])
-    Image.fromarray(out.cpu().numpy()).save(out_path)
-    return out
+    of it (the script passes `model.module` users).  Writes the uint8 PNG to out_path and returns it on the device."""
+    return _run([img], [tgt], [size], model, device, "segm", [out_path], pad=False)[0]
 
 
 @torch.no_grad()
 def run_one_image_nearest(img, tgt, size, model, out_path, device):
     """COCO panoptic instance / COCO pose: as run_one_image, with a nearest resize.  Writes the uint8 PNG."""
-    from PIL import Image
-    y, h, w, p = _predict(img, tgt, model, device)
-    out = nearest_u8(denorm_bottom(y, h, w, p, CLIP255), size[1], size[0])
-    Image.fromarray(out.cpu().numpy()).save(out_path)
-    return out
+    return _run([img], [tgt], [size], model, device, "nearest", [out_path], pad=False)[0]
 
 
 @torch.no_grad()
 def run_one_image_depth(img, tgt, size, model, out_path, device):
     """NYUv2 depth: clip(x * 10000, 0, 10000), bilinear, mean over the channels, int32.  Writes the int32 PNG (depth
     in units of 1e-4)."""
-    from PIL import Image
-    y, h, w, p = _predict(img, tgt, model, device)
-    out = depth_finish(denorm_bottom(y, h, w, p, CLIP10000), size[1], size[0])
-    Image.fromarray(out.cpu().numpy()).save(out_path)
-    return out
+    return _run([img], [tgt], [size], model, device, "depth", [out_path], pad=False)[0]
 
 
 @torch.no_grad()
@@ -139,11 +58,10 @@ def run_one_image_restore(img, tgt, size, model, out_path, device):
     """SIDD denoising / LoL enhancement / deraining: the de-normalised prediction, bicubic-resized, unclipped.
     Returns the float64 numpy array [height, width, 3] (the caller clips it and scores it); out_path is unused, as in
     the reference."""
-    y, h, w, p = _predict(img, tgt, model, device)
-    return bicubic_f64(denorm_bottom(y, h, w, p, PLAIN), size[1], size[0]).cpu().numpy()
+    return _run([img], [tgt], [size], model, device, "restore", None, pad=False)[0]
 
 
-# run_batch task -> (the run_one_image* it batches, pk_denorm_bottom finish, pk_finish_ragged op)
+# run_batch task -> (the run_one_image* it batches, pk_denorm_bottom_batched finish, pk_finish_ragged op)
 TASKS = {
     "segm": ("run_one_image", CLIP255, _se.FIN_BILINEAR_U8),
     "nearest": ("run_one_image_nearest", CLIP255, _se.FIN_NEAREST_U8),
@@ -153,7 +71,9 @@ TASKS = {
 
 
 def _cl_form(task, OH, OW):
-    """torch-CPU's kernel choice of the single-image wrapper (nearest_u8, depth_finish) for one output size."""
+    """pk_finish_ragged's cl_form for one output size: whether torch-CPU's F.interpolate of the 3-channel image takes
+    its channels-last kernel, whose nearest source index and bilinear tap order differ from its generic kernel's.  It
+    does for OH + OW <= 128 and, for the depth task's bilinear resize, on one thread."""
     if task == "nearest":
         return int(OH + OW <= 128)
     if task == "depth":
@@ -171,13 +91,18 @@ def run_batch(imgs, tgts, sizes, model, device, task, out_paths=None):
     One upload (canvases + descriptor table), one graphed forward, one de-normalise launch, one ragged resize launch,
     one download.  A batch smaller than one already captured for this canvas shape is padded to it by repeating the
     last canvas (the padding is dropped), so a dataset's tail batch replays the same CUDA graph."""
+    return _run(imgs, tgts, sizes, model, device, task, out_paths, pad=True)
+
+
+def _run(imgs, tgts, sizes, model, device, task, out_paths, pad):
+    """run_batch, with a forward of exactly len(imgs) canvases unless pad."""
     if task not in TASKS:
         raise ValueError(f"run_batch: task must be one of {sorted(TASKS)}, got {task!r}")
     B = len(imgs)
     if B < 1 or len(tgts) != B or len(sizes) != B or (out_paths is not None and len(out_paths) != B):
         raise ValueError(f"run_batch: {B} canvases, {len(tgts)} targets, {len(sizes)} sizes")
-    x = np.stack([np.asarray(a) for a in imgs])
-    t = np.stack([np.asarray(a) for a in tgts])
+    # one canvas stays a view: upload copies it into its pinned buffer, and a stack would copy it first
+    x, t = (np.asarray(c[0])[None] if B == 1 else np.stack([np.asarray(a) for a in c]) for c in (imgs, tgts))
     if x.dtype not in (np.float32, np.float64) or t.dtype != x.dtype or x.shape != t.shape or x.shape[-1] != 3:
         raise ValueError(f"run_batch: canvases {x.shape} {x.dtype} / targets {t.shape} {t.dtype}")
     _, finish, op = TASKS[task]
@@ -190,7 +115,7 @@ def run_batch(imgs, tgts, sizes, model, device, task, out_paths=None):
     p = net.patch_size
     h, w = H // p, W // p
     g = _graphed(net)
-    Bc = g.captured_batch((B, 3, H, W), B)
+    Bc = g.captured_batch((B, 3, H, W), B) if pad else B
     _se.precheck_memory(net, Bc, H, W)
     xin = torch.empty((Bc, 3, H, W), dtype=torch.float32, device=device)
     tin = torch.empty((Bc, 3, H, W), dtype=torch.float32, device=device)

@@ -6,11 +6,11 @@
 
 with identical arguments and results, but with everything between the decoded uint8 pixels and the finished uint8
 frame on the GPU: stitch + ImageNet normalisation + nhwc->nchw (pk_stitch_normalize), the forward (one CUDA-graph
-replay, painter_b200/graphs.py), unpatchify + bottom half + de-normalisation + clip (pk_seg_postprocess), nearest
-resize to the source size + alpha blend (pk_nearest_blend).  Image / video decoding, PIL resizing to 448x448 and file
-output stay on the host (file I/O is out of scope, SURVEY §2 row 5); the video path keeps its rolling prompt cache
-(previous frames and their binarised predictions, seggpt_engine.py:13-23,128-171) resident in HBM, so a frame costs
-one 0.6 MB upload however many cached prompts vote on it.
+replay, painter_b200/graphs.py), unpatchify + bottom half + de-normalisation + clip (pk_denorm_bottom_batched),
+nearest resize to the source size + alpha blend (pk_finish_ragged).  Image / video decoding, PIL resizing to 448x448
+and file output stay on the host (file I/O is out of scope, SURVEY §2 row 5); the video path keeps its rolling
+prompt cache (previous frames and their binarised predictions, seggpt_engine.py:13-23,128-171) resident in HBM, so a
+frame costs one 0.6 MB upload however many cached prompts vote on it.
 """
 import ctypes
 
@@ -70,21 +70,10 @@ def stitch_normalize(tops, bottoms, S):
     return out
 
 
-def seg_postprocess(patch, h, w, p, want_bin=False):
-    """patchified prediction [B, h*w, p*p*3] fp32 -> (fp64 [h*p/2, w*p, 3] in [0, 255], optional fp32 {0,1} mask)."""
-    assert patch.dtype == torch.float32 and patch.is_contiguous()
-    out = torch.empty((h * p // 2, w * p, 3), dtype=torch.float64, device=patch.device)
-    b = torch.empty((h * p // 2, w * p), dtype=torch.float32, device=patch.device) if want_bin else None
-    check(lib().pk_seg_postprocess(ctypes.c_void_p(patch.data_ptr()), ctypes.c_void_p(out.data_ptr()),
-                                   ctypes.c_void_p(b.data_ptr()) if b is not None else None, h, w, p, _stream()),
-          "pk_seg_postprocess")
-    return out, b
-
-
 def denorm_bottom_batched(patch, B, h, w, p, finish=0, src_stride=1, want_bin=False):
     """patchified prediction [*, h*w, p*p*3] fp32 -> fp64 [B, h*p/2, w*p, 3]: the bottom half of samples 0, src_stride,
     2 src_stride, .. de-normalised, then x255 clipped (finish 0), x10000 clipped (1) or left as is (2); optional fp32
-    {0,1} mask [B, h*p/2, w*p] (finish 0 only).  Sample b is what seg_postprocess / denorm_bottom give for it alone."""
+    {0,1} mask [B, h*p/2, w*p] (finish 0 only).  Sample b is what a B = 1 call on sample b * src_stride alone gives."""
     assert patch.dtype == torch.float32 and patch.is_contiguous() and patch.shape[0] >= (B - 1) * src_stride + 1
     out = torch.empty((B, h * p // 2, w * p, 3), dtype=torch.float64, device=patch.device)
     b = torch.empty((B, h * p // 2, w * p), dtype=torch.float32, device=patch.device) if want_bin else None
@@ -154,24 +143,13 @@ def upload(arrays, device):
         _staging[device] = ent
     host, done = ent
     done.synchronize()          # the previous transfer out of the pinned buffer has finished
-    hv = host.numpy()
-    for a, o in zip(arrays, offs):
-        hv[o:o + a.nbytes] = a.reshape(-1).view(np.uint8)
+    for a, o in zip(arrays, offs):      # torch copies on its intra-op threads, a numpy assignment on one
+        host[o:o + a.nbytes].copy_(torch.from_numpy(a.reshape(-1).view(np.uint8)))
     dev = torch.empty((max(n, 1),), dtype=torch.uint8, device=device)
     dev.copy_(host[:max(n, 1)], non_blocking=True)
     done.record()
     return [dev[o:o + a.nbytes].view(torch.from_numpy(a[:0].reshape(-1)).dtype).view(a.shape)
             for a, o in zip(arrays, offs)]
-
-
-def nearest_blend(seg, image_u8):
-    """seg fp64 [SH, SW, 3] (0..255), image uint8 [OH, OW, 3] (device) -> uint8 [OH, OW, 3] blended overlay."""
-    OH, OW, _ = image_u8.shape
-    dst = torch.empty_like(image_u8)
-    check(lib().pk_nearest_blend(ctypes.c_void_p(seg.data_ptr()), seg.shape[0], seg.shape[1],
-                                 ctypes.c_void_p(image_u8.data_ptr()), ctypes.c_void_p(dst.data_ptr()), OH, OW,
-                                 _stream()), "pk_nearest_blend")
-    return dst
 
 
 def _half_mask(model, device):
@@ -217,8 +195,8 @@ def run_one_image(img, tgt, model, device):
                                         ctypes.c_void_p(dst.data_ptr()), P, H, W, _stream()), "pk_nhwc_to_nchw_f32")
     y = _forward(model, xin, tin, device)
     p = model.patch_size
-    out, _ = seg_postprocess(y, H // p, W // p, p)
-    return out.cpu()
+    out, _ = denorm_bottom_batched(y, 1, H // p, W // p, p)
+    return out[0].cpu()
 
 
 def _load_prompt(img2_path, tgt2_path, res, hres, device):
@@ -233,13 +211,8 @@ def segment(model, device, image_u8, prompts, want_bin=False):
     """image_u8: device uint8 [448, 448, 3] (the query, resized); prompts: list of (prompt image, prompt target)
     device tensors [448, 448, 3] (uint8, or float in [0,1] for cached video frames).  Returns (fp64 [448, 448, 3] in
     [0, 255], optional binarised mask) - seggpt_engine.py:65-93 without the host arithmetic."""
-    S = image_u8.shape[0]
-    x = stitch_normalize([p[0] for p in prompts], [image_u8] * len(prompts), S)
-    t = stitch_normalize([p[1] for p in prompts], [p[1] for p in prompts], S)      # "tgt is not available"
-    torch.manual_seed(2)      # seggpt_engine.py:91 (no random op follows in eval mode; kept for RNG-state parity)
-    y = _forward(model, x, t, device)
-    p = model.patch_size
-    return seg_postprocess(y, 2 * S // p, S // p, p, want_bin=want_bin)
+    out, binm = _segment(model, device, [image_u8], prompts, want_bin, pad=False)
+    return out[0], None if binm is None else binm[0]
 
 
 @torch.no_grad()
@@ -249,19 +222,25 @@ def segment_batch(model, device, images_u8, prompts, want_bin=False):
     segment().  Returns (fp64 [Q, 448, 448, 3], optional mask [Q, 448, 448]); entry q equals segment(..., images_u8[q],
     prompts, want_bin) bit for bit.  A batch smaller than one already captured is padded to it by repeating the last
     query (its whole prompt group), so a folder runs on one CUDA graph; the padding is dropped."""
-    device = torch.device(device)
     Q, P = len(images_u8), len(prompts)
     if Q < 1 or P < 1:
         raise ValueError(f"segment_batch: {Q} queries, {P} prompts")
+    return _segment(model, device, images_u8, prompts, want_bin, pad=True)
+
+
+@torch.no_grad()
+def _segment(model, device, images_u8, prompts, want_bin, pad):
+    """segment_batch, with a forward of exactly len(images_u8) queries unless pad."""
+    device = torch.device(device)
+    Q, P = len(images_u8), len(prompts)
     S = images_u8[0].shape[0]
     p = model.patch_size
-    g = _graphed(model)
-    Qc = g.captured_batch((Q * P, 3, 2 * S, S), Q * P, P if P > 1 else None) // P
+    Qc = _graphed(model).captured_batch((Q * P, 3, 2 * S, S), Q * P, P if P > 1 else None) // P if pad else Q
     qs = [images_u8[q] for q in range(Q)] + [images_u8[Q - 1]] * (Qc - Q)
     precheck_memory(model, Qc * P, 2 * S, S)
     x = stitch_normalize([pr[0] for _ in qs for pr in prompts], [q for q in qs for _ in prompts], S)
     t = stitch_normalize([pr[1] for _ in qs for pr in prompts], [pr[1] for _ in qs for pr in prompts], S)
-    torch.manual_seed(2)      # as segment(): seggpt_engine.py:91, once per forward
+    torch.manual_seed(2)      # seggpt_engine.py:91 (no random op follows in eval mode; kept for RNG-state parity)
     y = _forward(model, x, t, device, P)
     # query q is member q * P's bottom half (seggpt_engine.py:48 takes member 0 of its batch)
     return denorm_bottom_batched(y, Q, 2 * S // p, S // p, p, 0, src_stride=P, want_bin=want_bin)
@@ -275,7 +254,8 @@ def precheck_memory(model, B, H, W):
         return
     need = accurate.workspace_bytes(model, B, H, W)
     free, _ = torch.cuda.mem_get_info()
-    free += torch.cuda.memory_reserved() - torch.cuda.memory_allocated()
+    if need > free:     # each of these builds the allocator's whole statistics dict: read them only when they matter
+        free += torch.cuda.memory_reserved() - torch.cuda.memory_allocated()
     if need > free:
         per = accurate.workspace_bytes(model, 1, H, W)
         raise RuntimeError(f"painter_b200: an fp32-accurate forward of {B} canvases of {H} x {W} needs about "
@@ -283,41 +263,45 @@ def precheck_memory(model, B, H, W):
                            f"{max(1, int(free // per))} canvases, or model.precision = 'bf16'")
 
 
+def _blend(model, device, images, prompts, pad):
+    """The queries' segmentations blended onto them at their own sizes (seggpt_engine.py:65-102): images are Q decoded
+    RGB PIL images.  One upload (the resized queries, the source images and the blend's descriptor table), one
+    forward (padded as in segment_batch if pad), one ragged blend launch.  Returns (packed uint8 device output, element
+    offset of every image in it)."""
+    srcs = [np.array(im) for im in images]
+    small = np.stack([np.array(im.resize((448, 448))) for im in images])
+    tab, offs, total, max_pix = ragged_table(FIN_NEAREST_BLEND, range(len(srcs)), [a.shape[:2] for a in srcs])
+    flat = np.concatenate([a.reshape(-1) for a in srcs])
+    small_d, flat_d, tab_d = upload([small, flat, tab], device)
+    out, _ = _segment(model, device, small_d, prompts, want_bin=False, pad=pad)
+    return finish_ragged(FIN_NEAREST_BLEND, out, tab_d, len(srcs), max_pix, total, image=flat_d), offs
+
+
 def inference_images(model, device, img_paths, img2_paths, tgt2_paths, out_paths, batch_size=8):
     """inference_image() over a folder of queries sharing one prompt set, batch_size queries per forward: writes the
-    same PNG files as one inference_image call per query.  Per batch: one upload (the resized queries, the source
-    images and the blend's descriptor table), one forward, one ragged blend launch, one download."""
+    same PNG files as one inference_image call per query.  Per batch: one upload, one forward, one ragged blend launch,
+    one download."""
     from PIL import Image
     device = torch.device(device)
     if len(img_paths) != len(out_paths) or batch_size < 1:
         raise ValueError("inference_images: one output path per query image, batch_size >= 1")
-    res, hres = 448, 448
-    prompts = [_load_prompt(a, b, res, hres, device) for a, b in zip(img2_paths, tgt2_paths)]
+    prompts = [_load_prompt(a, b, 448, 448, device) for a, b in zip(img2_paths, tgt2_paths)]
     for b0 in range(0, len(img_paths), batch_size):
         images = [Image.open(pth).convert("RGB") for pth in img_paths[b0:b0 + batch_size]]
-        srcs = [np.array(im) for im in images]
-        small = np.stack([np.array(im.resize((res, hres))) for im in images])
-        Q = len(images)
-        tab, offs, total, max_pix = ragged_table(FIN_NEAREST_BLEND, range(Q), [a.shape[:2] for a in srcs])
-        flat = np.concatenate([a.reshape(-1) for a in srcs])
-        small_d, flat_d, tab_d = upload([small, flat, tab], device)
-        out, _ = segment_batch(model, device, small_d, prompts)
-        blended = finish_ragged(FIN_NEAREST_BLEND, out, tab_d, Q, max_pix, total, image=flat_d).cpu().numpy()
-        for q in range(Q):
-            h, w = srcs[q].shape[:2]
-            Image.fromarray(blended[offs[q]:offs[q] + h * w * 3].reshape(h, w, 3)).save(out_paths[b0 + q])
+        blended, offs = _blend(model, device, images, prompts, pad=True)
+        host = blended.cpu().numpy()
+        for q, (im, o) in enumerate(zip(images, offs)):
+            h, w = im.height, im.width
+            Image.fromarray(host[o:o + h * w * 3].reshape(h, w, 3)).save(out_paths[b0 + q])
 
 
 def inference_image(model, device, img_path, img2_paths, tgt2_paths, out_path):
     from PIL import Image
     device = torch.device(device)
-    res, hres = 448, 448
     image = Image.open(img_path).convert("RGB")
-    input_image = torch.from_numpy(np.array(image)).to(device)
-    image_r = torch.from_numpy(np.array(image.resize((res, hres)))).to(device)
-    prompts = [_load_prompt(a, b, res, hres, device) for a, b in zip(img2_paths, tgt2_paths)]
-    out, _ = segment(model, device, image_r, prompts)
-    blended = nearest_blend(out, input_image)
+    prompts = [_load_prompt(a, b, 448, 448, device) for a, b in zip(img2_paths, tgt2_paths)]
+    blended, _ = _blend(model, device, [image], prompts, pad=False)
+    blended = blended.view(image.height, image.width, 3)
     Image.fromarray(blended.cpu().numpy()).save(out_path)
     return blended
 
@@ -342,6 +326,7 @@ def inference_video(model, device, vid_path, num_frames, img2_paths, tgt2_paths,
     tgt2 = Image.open(tgt2_paths[0]).convert("RGB").resize((res, hres), Image.NEAREST)
     tgt2 = torch.from_numpy(np.array(tgt2)).to(device)
     frames_cache, target_cache = Cache(num_frames), Cache(num_frames)
+    tab_d = None
     n = 0
     while True:
         ret, frame = cap.read()
@@ -349,14 +334,20 @@ def inference_video(model, device, vid_path, num_frames, img2_paths, tgt2_paths,
             break
         image = Image.fromarray(frame[:, :, ::-1]).convert('RGB')
         input_image = torch.from_numpy(np.array(image)).to(device)
+        if tab_d is None:       # one blend table for the whole video
+            hw = input_image.shape[:2]
+            tab, _, total, max_pix = ragged_table(FIN_NEAREST_BLEND, [0], [hw])
+            tab_d = torch.from_numpy(tab).to(device)
+        elif input_image.shape[:2] != hw:
+            raise ValueError(f"inference_video: frame {n} is {tuple(input_image.shape[:2])}, frame 0 {tuple(hw)}")
         image_r = torch.from_numpy(np.array(image.resize((res, hres)))).to(device)
         prompts = list(zip([img2] + frames_cache, [tgt2] + target_cache))
         out, binm = segment(model, device, image_r, prompts, want_bin=num_frames > 0)
         frames_cache.append(image_r)
         if num_frames > 0:
             target_cache.append(binm.unsqueeze(-1).expand(-1, -1, 3).contiguous())
-        blended = nearest_blend(out, input_image)
-        video_writer.write(np.ascontiguousarray(blended.cpu().numpy()[:, :, ::-1]))
+        blended = finish_ragged(FIN_NEAREST_BLEND, out.unsqueeze(0), tab_d, 1, max_pix, total, image=input_image)
+        video_writer.write(np.ascontiguousarray(blended.view(input_image.shape).cpu().numpy()[:, :, ::-1]))
         n += 1
     video_writer.release()
     return n

@@ -89,6 +89,23 @@ def test_denorm_bottom_batched_argument_validation(lib):
     _refused(L, call(bin_ptr=NZ, finish=2), "binarised mask")
 
 
+def test_single_image_finishing_entry_points_are_not_exported(lib):
+    """Every finishing step goes through pk_denorm_bottom_batched and pk_finish_ragged, for one image as for many."""
+    for name in ("seg_postprocess", "denorm_bottom", "nearest_blend", "bilinear_u8", "bicubic_f64", "depth_finish",
+                 "nearest_u8"):
+        assert not hasattr(lib, "pk_" + name), name
+
+
+@pytest.mark.parametrize("dtype", [np.float16, np.int32])
+def test_painter_mirrors_refuse_canvases_that_are_not_float32_or_float64(dtype):
+    """Refused before any device work, as run_batch refuses them, instead of being read as float32."""
+    from painter_b200 import painter_inference as pi
+    x = np.zeros((896, 448, 3), dtype)
+    for mirror in ("run_one_image", "run_one_image_nearest", "run_one_image_depth", "run_one_image_restore"):
+        with pytest.raises(ValueError, match="canvases"):
+            getattr(pi, mirror)(x, x, (10, 10), None, "unused.png", "cuda")
+
+
 def test_stitch_normalize_checks_every_member(lib):
     """Any number of members is accepted (launched in chunks of 16); each member is still checked."""
     L = lib

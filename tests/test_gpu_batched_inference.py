@@ -4,8 +4,8 @@ per-image mirrors, bit for bit.
 The mirrors are pinned to the unmodified reference functions (test_gpu_inference.py, test_gpu_painter_tasks.py), so
 equality with them carries that parity over.  Equality holds because no forward computation mixes samples in a way
 that depends on the batch size (forward GEMMs never split K, attention is per (sample, head), LayerNorm per row, the
-fp32-accurate decoder runs one image at a time, the prompt ensemble averages over one query's own members) and the
-batched finishing kernels run the single-image kernels' per-pixel code.  Everything runs at the full 896 x 448
+fp32-accurate decoder runs one image at a time, the prompt ensemble averages over one query's own members) and every
+image of a finishing launch gets the same per-pixel code.  Everything runs at the full 896 x 448
 geometry with seeded random weights, in the fp32-accurate mode ("auto" under no_grad, what the mirrors select) and in
 bf16."""
 import numpy as np
@@ -188,7 +188,10 @@ def test_inference_images_writes_the_same_files(seggpt, tmp_path):
         assert open(a, "rb").read() == open(b, "rb").read(), b
 
 
-def test_ragged_kernels_equal_single_image_kernels():
+def test_ragged_launch_equals_one_image_launches():
+    """Each image of one n-image pk_finish_ragged launch equals, bit for bit, a one-row launch of that image alone
+    (its source sample as the only one, output at offset 0): the rows' source samples, output offsets and per-row
+    cl_form are addressed right.  Likewise each sample of a strided pk_denorm_bottom_batched launch, mask included."""
     from painter_b200 import painter_inference as pi
     from painter_b200 import seggpt_engine as se
     torch.manual_seed(0)
@@ -198,33 +201,35 @@ def test_ragged_kernels_equal_single_image_kernels():
     sizes = [(427, 640), (523, 301), (50, 60), (58, 71), (9, 13), (448, 448), (896, 896)]    # (OH, OW)
     srcs = [k % B for k in range(len(sizes))]
     images = [torch.randint(0, 256, (oh, ow, 3), dtype=torch.uint8, device="cuda") for oh, ow in sizes]
-    single = {
-        se.FIN_BILINEAR_U8: (src, lambda s, oh, ow, k: pi.bilinear_u8(s, oh, ow), lambda oh, ow: 0),
-        se.FIN_NEAREST_U8: (src, lambda s, oh, ow, k: pi.nearest_u8(s, oh, ow), lambda oh, ow: int(oh + ow <= 128)),
-        se.FIN_DEPTH: (depth_src, lambda s, oh, ow, k: pi.depth_finish(s, oh, ow),
-                       lambda oh, ow: int(torch.get_num_threads() == 1 or oh + ow <= 128)),
-        se.FIN_BICUBIC_F64: (src, lambda s, oh, ow, k: pi.bicubic_f64(s, oh, ow), lambda oh, ow: 0),
-        se.FIN_NEAREST_BLEND: (src, lambda s, oh, ow, k: se.nearest_blend(s, images[k]), lambda oh, ow: 0),
+    ops = {    # op -> (source, torch-CPU's cl_form for an output size)
+        se.FIN_BILINEAR_U8: (src, lambda oh, ow: 0),
+        se.FIN_NEAREST_U8: (src, lambda oh, ow: int(oh + ow <= 128)),
+        se.FIN_DEPTH: (depth_src, lambda oh, ow: int(torch.get_num_threads() == 1 or oh + ow <= 128)),
+        se.FIN_BICUBIC_F64: (src, lambda oh, ow: 0),
+        se.FIN_NEAREST_BLEND: (src, lambda oh, ow: 0),
     }
-    for op, (base, fn, cl) in single.items():
+    for op, (base, cl) in ops.items():
+        blend = op == se.FIN_NEAREST_BLEND
         tab, offs, total, max_pix = se.ragged_table(op, srcs, sizes, [cl(oh, ow) for oh, ow in sizes])
-        tab_d = torch.from_numpy(tab).cuda()
-        img = torch.cat([i.reshape(-1) for i in images]) if op == se.FIN_NEAREST_BLEND else None
-        out = se.finish_ragged(op, base, tab_d, len(sizes), max_pix, total, image=img)
+        img = torch.cat([i.reshape(-1) for i in images]) if blend else None
+        out = se.finish_ragged(op, base, torch.from_numpy(tab).cuda(), len(sizes), max_pix, total, image=img)
         for k, (oh, ow) in enumerate(sizes):
-            ref = fn(base[srcs[k]], oh, ow, k).reshape(-1)
-            assert torch.equal(out[offs[k]:offs[k] + ref.numel()], ref), (op, k, oh, ow)
-    # batched de-normalisation (with the binarised mask) vs the single-image call on each sample
+            tab1, _, total1, max_pix1 = se.ragged_table(op, [0], [(oh, ow)], [cl(oh, ow)])
+            ref = se.finish_ragged(op, base[srcs[k]:srcs[k] + 1], torch.from_numpy(tab1).cuda(), 1, max_pix1, total1,
+                                   image=images[k] if blend else None)
+            assert torch.equal(out[offs[k]:offs[k] + total1], ref), (op, k, oh, ow)
+    # strided batched de-normalisation (with the binarised mask) vs a one-sample launch on each sample
     p, h, w = 16, 56, 28
     patch = torch.randn(5, h * w, p * p * 3, device="cuda")
     for finish in (pi.CLIP255, pi.CLIP10000, pi.PLAIN):
-        out, binm = se.denorm_bottom_batched(patch, 3, h, w, p, finish, src_stride=2,
-                                             want_bin=finish == pi.CLIP255)
+        want_bin = finish == pi.CLIP255
+        out, binm = se.denorm_bottom_batched(patch, 3, h, w, p, finish, src_stride=2, want_bin=want_bin)
         for b in range(3):
-            assert torch.equal(out[b], pi.denorm_bottom(patch[2 * b:2 * b + 1].contiguous(), h, w, p, finish))
-            if finish == pi.CLIP255:
-                ref, rbin = se.seg_postprocess(patch[2 * b:2 * b + 1].contiguous(), h, w, p, want_bin=True)
-                assert torch.equal(out[b], ref) and torch.equal(binm[b], rbin)
+            ref, rbin = se.denorm_bottom_batched(patch[2 * b:2 * b + 1].contiguous(), 1, h, w, p, finish,
+                                                 want_bin=want_bin)
+            assert torch.equal(out[b], ref[0]), (finish, b)
+            if want_bin:
+                assert torch.equal(binm[b], rbin[0]), b
 
 
 def test_tail_batch_replays_one_graph(painter, tmp_path):

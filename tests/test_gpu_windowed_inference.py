@@ -130,9 +130,9 @@ def test_seggpt_tiny_window_ensemble_fp32_and_bf16():
         assert lb <= LOSS_TOL and pb <= LOGIT_RMS, (c["P"], c["merge_between_batch"], lb, pb)
 
 
-def test_seggpt_tiny_window_graph_replay_matches_eager():
+def test_seggpt_tiny_window_graph_replay_matches_eager_denorm():
     """seggpt_engine.run_one_image replays the forward as a CUDA graph; with P = 2 it runs the windowed blocks with the
-    ensemble in the fp32-accurate mode.  Same result as an eager forward + the same post-processing."""
+    ensemble in the fp32-accurate mode.  Same result as an eager forward + a one-sample denorm_bottom_batched."""
     from painter_b200 import seggpt_engine
     gold, cfg, model = _seggpt_window()
     model.seg_type = "semantic"
@@ -147,8 +147,8 @@ def test_seggpt_tiny_window_graph_replay_matches_eager():
     bm[:, h * w // 2:] = 1
     with torch.no_grad():
         _, y, _ = model(x.cuda(), t.cuda(), bm, torch.ones_like(t).cuda(), torch.zeros(2, 1, device="cuda"), 0)
-        out_e, _ = seggpt_engine.seg_postprocess(y, h, w, p)
-    out_e = out_e.cpu()
+        out_e, _ = seggpt_engine.denorm_bottom_batched(y, 1, h, w, p)
+    out_e = out_e[0].cpu()
     tol = 1e-6 * out_e.abs().max().item()
     assert (out_g - out_e).abs().max().item() <= tol
     assert (out_g2 - out_e).abs().max().item() <= tol
